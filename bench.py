@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """bench.py - IQ Msamples/s of the composite-video -> IQ hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch: FRAMES video frames (default 1024 =
 640 000 scan lines = 655 M complex samples, rendered in 16 calls of 64 frames = 164 MB of
-int16 IQ each - larger than the 126 MB L2 - into the same device buffer; 20 steps keep the
+int16 IQ each - larger than the 50 MB L2 of an H100 - into the same device buffer; 20 steps keep the
 GPU busy for > 100 ms, so the 1 kHz clock sampler sees the timed region) of BASELINE config 2: PAL System I, 16 Msps, --filter (VSB) + FM mono + NICAM-728 +
 colour, built-in test pattern and tone. With N GPUs each rank renders its own independent
 RF channel on its own GPU (weak scaling, no collective on the data path); `value` is
@@ -14,8 +14,8 @@ the sum over channels divided by the slowest rank's device time.
 Keys beyond the base contract:
   roofline      HBM-write roofline of the dominant kernel (k_line, the fused line kernel):
                 algorithmic bytes (4 B per complex sample) / CUDA-event duration of that
-                kernel, vs the measured copy bandwidth in MEASURED_PEAKS.json; step_frac is
-                the same for the whole step, issue the kernel's issue-slot figures from ncu.
+                kernel, vs the measured copy bandwidth in MEASURED_PEAKS.json (else the H100 SXM
+                data-sheet figure); step_frac is the same for the whole step.
   extra         device-resident lines for the other BASELINE configs (1, 3, 4, 5) and, at
                 N = 1, the drop-in path: hacktv's own CLI on the adapter vs the stock CLI.
   e2e           the same metric through htv_render_host() with HOST buffers: every
@@ -23,6 +23,12 @@ Keys beyond the base contract:
                 renders, and copies the IQ back to pinned host memory.
   cpu_baseline  the UNMODIFIED reference (oracle/_ref/ref_harness) timed on this box's
                 host cores on a bounded sample of the same workload (rank 0, N = 1 only).
+
+--dump-outputs DIR writes what the timed path computed in its last call, as the caller receives it: a fixed,
+seeded sample of DUMP_LINES scan lines of int16 IQ as float32 (DIR/iq.npy, [lines, values per line]: I and Q
+interleaved, or I alone for real output) with their line numbers in the stream (DIR/iq_lines.npy, float64), and the same for the
+last end-to-end step (DIR/e2e_iq.npy, DIR/e2e_iq_lines.npy). The inputs are the built-in test source, so the
+same arguments give the same inputs on every run and two builds can be compared output for output.
 
 --impl reference times the reference's own CPU implementation with every host thread it
 can use (as many concurrent encoder instances as fit; one instance = 1 + nthreads
@@ -48,10 +54,7 @@ WORKLOADS = {   # --workload: the metric is quoted on cfg2; cfg5 is BASELINE con
 CHUNK_FRAMES = 64        # frames per htv_render call: 164 MB of IQ at 16 Msps, larger than the L2
 REF_HARNESS = os.path.join(ROOT, "oracle", "_ref", "ref_harness")
 REF_THREADS = 3          # main/raster + vfilter + audio (reference video.c:4692: 1 + nthreads)
-# From the ncu --set full capture of the shipped k_line (profiles/r02_summary.md), per scan line of 1024 samples:
-# dram__bytes_read.sum + dram__bytes_write.sum of one launch over 40 000 lines, and the issue-slot figures.
-NCU = {"file": "profiles/r02_ncu_k_line_raw.txt", "lines": 40000, "dram_read": 47_632_128, "dram_write": 113_646_080,
-       "warp_instructions": 238_153_871, "issue_active_pct": 61.8}
+DUMP_LINES = 2048        # scan lines per --dump-outputs array: 16.8 MB as float32 at 1024 complex samples per line
 KERNEL = "k_line (fused line kernel: raster + chroma and video filters on the tensor cores + sound carriers + IQ store)"
 
 
@@ -60,11 +63,11 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md) through
+    """SM clock and throttle reasons sampled DURING the timed region through
     NVML at ~1 kHz (the region is only milliseconds long; spawning nvidia-smi is too slow).
     Falls back to one nvidia-smi query if NVML is unavailable."""
 
@@ -86,6 +89,12 @@ class ClockSampler:
             self._max = pynvml.nvmlDeviceGetMaxClockInfo(self._h, pynvml.NVML_CLOCK_SM)
         except Exception:
             self._nv = None
+        self.power_limit_w = None
+        if self._nv:
+            try:
+                self.power_limit_w = round(self._nv.nvmlDeviceGetEnforcedPowerLimit(self._h) / 1000.0, 1)
+            except Exception:
+                pass
 
     def _run(self):
         nv = self._nv
@@ -127,7 +136,8 @@ class ClockSampler:
                     if bit and (r[3] & bit):
                         reasons.add(k)
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max((r[2] for r in rows), default=None),
-                "reasons": sorted(reasons), "samples": len(rows), "source": "nvml" if nv else "nvidia-smi"}
+                "reasons": sorted(reasons), "samples": len(rows), "source": "nvml" if nv else "nvidia-smi",
+                "power_limit_w": self.power_limit_w}
 
 
 def cpu_budget():
@@ -291,6 +301,19 @@ def device_resident(H, torch, mode, rate, filt, frames, steps, warmup, stream, c
     return enc, out, chunk, calls, nsamp, l0, ev0, ev1
 
 
+def dump_sample(dump_dir, name, iq, nlines, first_line):
+    """`iq`: the int16 output of one call of nlines lines (torch tensor, device or host) whose first line is line
+    `first_line` of the stream. Writes a seeded sample of DUMP_LINES of its lines as float32, and their line numbers."""
+    import numpy as np
+    import torch
+    rows = np.sort(np.random.default_rng(2024).choice(nlines, size=min(nlines, DUMP_LINES), replace=False))
+    lines = iq[: iq.numel() // nlines * nlines].view(nlines, -1)
+    sample = lines[torch.from_numpy(rows).to(lines.device)].to(torch.float32).cpu().numpy()
+    os.makedirs(dump_dir, exist_ok=True)
+    np.save(os.path.join(dump_dir, name + ".npy"), sample)
+    np.save(os.path.join(dump_dir, name + "_lines.npy"), (rows + first_line).astype(np.float64))
+
+
 def quick_config(H, torch, stream, name, mode, rate, filt, frames=CHUNK_FRAMES, iters=10):
     """One device-resident line for a BASELINE config that is not the metric's workload (for `extra`)."""
     enc = H.Encoder(H.mode_config(mode, vfilter=filt), rate)
@@ -386,6 +409,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-extra", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write a sample of the last timed call's IQ as .npy files here")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -436,6 +460,10 @@ def main():
         clk.t1 = time.perf_counter()
     ms = ev0.elapsed_time(ev1)
     launches = enc.kernel_launches - l0
+    tag = "" if world == 1 else f"rank{rank}_"
+    if args.dump_outputs:
+        # `out` holds the last call of the last step; the warm-up rendered one call each
+        dump_sample(args.dump_outputs, tag + "iq", out, chunk, (args.warmup + args.steps * calls - 1) * chunk)
     clocks = clk.summary()
     # per-launch duration of the dominant kernel, CUDA events on its own stream (untimed extra steps)
     kern_ms = []
@@ -470,6 +498,8 @@ def main():
             enc2.render_host_ptr(e2e_lines, host.data_ptr())
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
+        if args.dump_outputs:
+            dump_sample(args.dump_outputs, tag + "e2e_iq", host, e2e_lines, (max(1, args.warmup) + args.steps - 1) * e2e_lines)
         e2e_samples = e2e_lines * enc2.width
         e2e_s, e2e_job = reduce_job(torch, dist, world, dt, e2e_samples * args.steps)
         h2d = e2e_frames * enc2.active_width * enc2.active_lines * 4 + int(e2e_samples / rate * 32000) * 4
@@ -506,7 +536,6 @@ def main():
                 quick_config(H, torch, stream, "cfg4: -m l -s 16000000 --filter (SECAM)", "l", 16_000_000, True),
                 quick_config(H, torch, stream, "cfg5 (one channel): -m i -s 20000000 --filter", "i", 20_000_000, True)],
                 "dropin_cli": dropin_throughput()}
-        per_line = 1.0 / NCU["lines"]
         emit({
             "metric": "IQ Msamples/s", "value": round(value, 2), "unit": "Msamples/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -515,23 +544,21 @@ def main():
             "config": {"workload": workload, "frames_per_step": calls * min(args.frames, CHUNK_FRAMES), "lines_per_step": nlines,
                        "calls_per_step": calls, "frames_per_call": min(args.frames, CHUNK_FRAMES),
                        "samples_per_step_per_gpu": step_samples, "parallelism": f"{world} independent RF channel(s), one per GPU, no collectives",
-                       "l2": f"every call writes {nsamp * 4 / 1e6:.0f} MB of IQ per GPU (> 126 MB L2); tables are L2-resident by design",
+                       "l2": f"every call writes {nsamp * 4 / 1e6:.0f} MB of IQ per GPU (> 50 MB L2); tables are L2-resident by design",
                        "ms_per_64_frames": round(ms_max / args.steps / calls, 4),
                        "realtime_x": round(value / world / (rate / 1e6), 1)},
             "roofline": {"bound": "hbm", "achieved": round(achieved, 1) if achieved else None, "peak": peak, "unit": "GB/s",
                          "frac": round(achieved / peak, 4) if achieved else None,
-                         "traffic": int(round((NCU["dram_read"] + NCU["dram_write"]) * per_line * kern_lines)) if width == 1024 else None,
                          "kernel": KERNEL, "kernel_ms": round(k_ms, 4),
                          "lines_per_launch": kern_lines, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": k_samples * 4,
                          "step_achieved": round(step_gbs, 1), "step_frac": round(step_gbs / peak, 4),
-                         "issue": {"slots_per_sample": round(NCU["warp_instructions"] * 32 / (NCU["lines"] * 1024), 1),
-                                   "issue_active_pct": NCU["issue_active_pct"], "source": NCU["file"]},
-                         "note": "4 B per complex sample written once; the kernel is issue-slot bound (DESIGN.md section 4), not HBM bound"},
+                         "note": "4 B per complex sample written once"},
             "cpu_baseline": cpu,
             "e2e": e2e,
             "gpu_launches": int(launches),
             "clocks": clocks,
+            "gpu": torch.cuda.get_device_name(local),
             "checksum": checksum,
             "extra": extra,
         })

@@ -1,6 +1,6 @@
 """hacktv_b200 - Python view of the C-ABI in include/hacktv_b200.h.
 
-The product is the shared library ``libhacktv_b200.so`` (C host layer + sm_100a
+The product is the shared library ``libhacktv_b200.so`` (C host layer + sm_90a
 CUDA kernels). This module only loads it with ctypes and mirrors the
 reference-facing call sequence (reference hacktv.c:1440-1601):
 
@@ -99,7 +99,7 @@ _lib = None
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the C host layer and the sm_100a kernels in-tree (csrc/Makefile)."""
+    """Compile the C host layer and the sm_90a kernels in-tree (csrc/Makefile)."""
     r = subprocess.run(["make", "-C", os.path.join(_HERE, "csrc")], capture_output=True, text=True)
     if verbose or r.returncode != 0:
         print(r.stdout[-4000:])

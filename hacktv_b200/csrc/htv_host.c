@@ -87,7 +87,7 @@ struct htv_t {
 
 static void drop_overlays_before(htv_t *s, long long line);
 
-const char *htv_version(void) { return("hacktv_b200 0.1 (sm_100a)"); }
+const char *htv_version(void) { return("hacktv_b200 0.1 (sm_90a)"); }
 
 const htv_config_t *htv_find_mode(const char *id)
 {
@@ -474,7 +474,7 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 					s->next_slot = (s->next_slot + 1) % MAX_FRAME_SLOTS;
 					/* pictures that follow each other in the caller's memory (a capture ring, htv_av_memory_open's array)
 					 * and land in consecutive slots go up as ONE copy: 2 MB copies beside the 8 MB copies coming back
-					 * keep neither PCIe direction full (measured: 4.4 ms for what full duplex moves in 3.1 ms) */
+					 * keep neither PCIe direction full */
 					if(run_n > 0 && fr.framebuffer == run_src + (size_t) run_n * fpix && s->cur_slot == run_slot + run_n) run_n++;
 					else
 					{
@@ -597,7 +597,7 @@ int htv_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalues, void *cuda_
 }
 
 /* copy-back granularity: small enough that the first render / last copy (which overlap nothing)
- * stay short, large enough for full PCIe rate (measured on the B200 box: 4-48 MB within 10 %) */
+ * stay short, large enough for full PCIe rate */
 #define HOST_PIECE_BYTES (8u << 20)
 
 /* On an error in the middle of the pipeline both streams are drained before returning, so no

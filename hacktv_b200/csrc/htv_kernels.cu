@@ -1,4 +1,4 @@
-// hacktv_b200 - CUDA kernels (sm_100a) and the device layer behind the C-ABI.
+// hacktv_b200 - CUDA kernels (sm_90a) and the device layer behind the C-ABI.
 //
 // One CTA renders one scan line; a launch covers a run of lines (a field, a
 // frame, or many frames). Every piece of state the reference carries from
@@ -2496,13 +2496,14 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 }
 
 // resident CTAs per SM of the persistent line kernels, by CTA size (256 / 320 / 384 threads <-> W <= 1024 / 1280 / 1536).
-// tools/occ_ab.sh builds and times the alternatives: 5 or 6 CTAs of 256 threads (48 / 40 registers) are 3 % / 10 % slower
-// than 4 (62 registers) - the compiler pays for the registers with instructions - while 4 CTAs of 320 threads beat 3.
+// tools/occ_ab.sh builds and times the alternatives. On an H100 SXM (700 W, 1980 MHz), ms per 64 frames: 3 CTAs of 256
+// threads instead of 4 take 0.509 against 0.493 at W = 1024 and 0.422 against 0.347 at W = 858; 3 CTAs of 320 threads
+// instead of 4 take 0.626 against 0.587 at W = 1280, although at 4 the compiler caps them at 48 registers and spills a little.
 #ifndef KL_B256
 #define KL_B256 4
 #endif
 #ifndef KL_B320
-#define KL_B320 4                     // 48 registers, no spills; measured against 3 (64 registers): 0.504 -> 0.481 ms per 64 frames at W = 1280
+#define KL_B320 4
 #endif
 #ifndef KL_B384
 #define KL_B384 2
@@ -2655,7 +2656,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	cudaFuncSetAttribute(k_raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->raster_smem);
 	cudaFuncSetAttribute(k_mod<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
 	cudaFuncSetAttribute(k_mod<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
-	// sub-batches keep the int16 composite scratch (2 B/sample) resident in the 126 MB L2
+	// sub-batches keep the int16 composite scratch (2 B/sample) resident in the 50 MB L2
 	const bool secam = dp.colour_mode == HTV_SECAM;
 	// SECAM: the cross-line chain is latency bound per launch, so one launch should cover the whole call
 	d->sub_lines = ((secam ? 160 : 16) * 1024 * 1024) / (W * 2);
@@ -2683,7 +2684,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	}
 	if(!secam && (W & 3) == 0 && !dp.have_fmv && !t->raster_only)
 	{
-		int nsm = 148;
+		int nsm = 132;
 		cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
 		d->modt_smem = sizeof(int) * 2 * TWIN(W) + 2 * sizeof(LineAudio) + sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
 		if(cudaMalloc((void **) &d->d_comp32, sizeof(int) * (((size_t) d->sub_lines + 3) * W + 256)) != cudaSuccess)
@@ -2712,13 +2713,13 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	{
 		// the video filter on the tensor cores (k_mod_mma), the default for every line width: multiples of
 		// 128 through the contiguous byte planes, the rest (NTSC 858, 864, ...) through the pitched plane
-		// layout (htv_mma_fir.h) - both validated against the scalar filter and the oracle on a B200
+		// layout (htv_mma_fir.h) - both validated against the scalar filter and the oracle
 		// (tests/test_gpu_zz_mma_fir.py). HTV_FIR=scalar selects the scalar kernels (A/B runs, tests)
 		const char *sel = getenv("HTV_FIR");
 		const bool want_mma = sel ? strcmp(sel, "scalar") != 0 : HTV_FIR_DEFAULT_MMA;
 		if(want_mma)
 		{
-			int nsm = 148;
+			int nsm = 132;
 			cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
 			d->mod_grid = nsm * (d->line_threads <= 256 ? 4 : 2);
 			uint32_t atab[MF_ATAB_WORDS];
@@ -2743,7 +2744,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	if(secam && !dp.have_fmv && !t->raster_only && !t->rs_taps && !(getenv("HTV_PATH") && !strcmp(getenv("HTV_PATH"), "split")))
 	{
 		// SECAM: raster and chrominance chain write the composite rows, the fused line kernel's SRC form modulates them
-		int nsm = 148;
+		int nsm = 132;
 		cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
 		if(dp.vf_type)
 		{
@@ -2801,7 +2802,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		const bool vf_ok = dp.vf_type == 0 || d->dt.mma_atab != NULL;
 		if(!split && !secam && !dp.have_fmv && !t->raster_only && !t->rs_taps && chroma_ok && vf_ok && dt.tmpl_out)
 		{
-			int nsm = 148;
+			int nsm = 132;
 			cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
 			const int T = mf_tiles(W);
 			d->kl_threads = 32 * T;
@@ -3549,7 +3550,7 @@ extern "C" int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalu
 {
 	if(!nvalues) return(HTV_OK);
 	if((((uintptr_t) d_acc) | ((uintptr_t) d_in)) & 15) return(HTV_ERROR);
-	int dev = 0, nsm = 148;
+	int dev = 0, nsm = 132;
 	cudaGetDevice(&dev);
 	{
 		// run where the accumulator lives (d_in may be peer memory)

@@ -1,4 +1,4 @@
-/* hacktv_b200 - the C-ABI of the B200-native composite-video -> IQ hot path.
+/* hacktv_b200 - the C-ABI of the H100-native composite-video -> IQ hot path.
  *
  * This header is the drop-in boundary. Everything here is `extern "C"`, plain
  * pointers and sizes; no CUDA, torch or C++ types appear in any signature

@@ -60,7 +60,7 @@ def test_frames_at_10s_and_34s_match_the_reference(built, name):
         tol = 1 + (int(np.ceil(0.35 * seconds)) if resonant else 0)
         # sound carriers are closed-form NCOs: +-1 LSB (BASELINE.json north_star); the rest is exact
         assert d.max() <= tol, f"{name} window {tag} (line {w['skip']}): max |diff| {d.max()} > {tol}, {np.count_nonzero(d > tol)} values out"
-        # measured on a B200: 0.88 (SECAM-L at 34 s: AM + NICAM carriers) .. 0.98 exact; a model error would show as a drop
+        # most values are exact (SECAM-L at 34 s, with AM + NICAM carriers, has the fewest); a model error would show as a drop
         if not resonant:
             assert (d == 0).mean() > 0.85, f"{name} window {tag}: only {(d == 0).mean():.3f} exact"
     enc.close()

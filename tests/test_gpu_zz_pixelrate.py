@@ -1,7 +1,7 @@
 """--pixelrate on the GPU (SURVEY.md section 8f rank 4): raster in a second device context at the pixel
 rate, k_resample (the reference's polyphase resampler in closed form), then the usual modulator - against the
 oracle, which is pinned bit for bit to the reference's own --pixelrate output (tests/test_oracle_vs_ref.py).
-First run on a B200 in round 2: every case within the stated tolerance on the first attempt."""
+"""
 import os
 
 import numpy as np

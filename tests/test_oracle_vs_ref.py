@@ -1,12 +1,31 @@
-"""The oracle against the reference itself (oracle/_ref/ref_harness, the unmodified
-fsphil/hacktv sources compiled in place): bit-exact, incl. inputs and options the golden
-fixtures do not cover. Skipped where the prebuilt reference is absent."""
+"""The oracle against the reference itself: bit-exact, incl. inputs and options the golden fixtures of
+test_oracle_golden.py do not cover. What the UNMODIFIED reference (the fsphil/hacktv sources compiled in place
+into oracle/_ref/ref_harness) emitted for each case is stored as a sha256 of its int16 stream in
+tests/golden/golden_ref.json, and the two scan lines the WSS overlay is recovered from in golden_ref_wss.npz;
+tests/golden/make_golden_ref.py runs the reference and writes both. No GPU and no reference tree needed."""
+import functools
+import hashlib
+import json
+import os
+
 import numpy as np
 import pytest
 
 import orc
 
-pytestmark = pytest.mark.skipif(not orc.have_ref(), reason="oracle/_ref not built (needs /root/reference at build time)")
+HERE = os.path.dirname(os.path.abspath(__file__))
+
+
+@functools.cache
+def golden_ref():
+    with open(os.path.join(HERE, "golden", "golden_ref.json")) as f:
+        return json.load(f)
+
+
+@functools.cache
+def golden_wss_lines():
+    return dict(np.load(os.path.join(HERE, "golden", "golden_ref_wss.npz")))
+
 
 CASES = [
     ("pal", 16000000, 700, False, ()),
@@ -38,6 +57,37 @@ CASES = [
 ]
 
 
+def ref_key(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", rawheap=False):
+    """Names one reference run in golden_ref.json: its command line, with the input it was given instead of file
+    names (`source`: the built-in test source, or which seeded random input / passthru stream)."""
+    parts = [f"-m {mode} -s {rate} --skip {skip} --lines {lines}"] + (["--filter"] if vfilter else []) + list(extra)
+    return " ".join(parts + [f"source={source}"] + (["rawheap"] if rawheap else []))
+
+
+def digest(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def assert_reference(got, key):
+    want = golden_ref()[key]
+    assert got.size == want["size"], (got.size, want["size"])
+    assert digest(got) == want["sha256"], f"the oracle's stream differs from the reference's ({key})"
+
+
+def passthru_stream(width, ext_lines, seed=11, tail=None):
+    """The external int16 IQ stream fed to --passthru (tail: complex samples past the last whole line)."""
+    rng = np.random.default_rng(seed)
+    return rng.integers(-32768, 32767, size=(ext_lines * width + (width // 3 if tail is None else tail), 2), dtype=np.int16)
+
+
+def random_source(seed, active_lines, active_width):
+    """Two random pictures and 30 000 random stereo sound samples (the reference reads the sound in blocks of 4000)."""
+    rng = np.random.default_rng(seed)
+    frames = rng.integers(0, 1 << 24, size=(2, active_lines, active_width), dtype=np.uint32)
+    audio = rng.integers(-32768, 32767, size=(30000, 2), dtype=np.int16)
+    return frames, audio
+
+
 def _conf(H, mode, filt, extra):
     kw = dict(vfilter=filt)
     it = iter(extra)
@@ -56,9 +106,7 @@ def test_oracle_equals_reference(built, mode, rate, nlines, filt, extra):
     o.open_test_source()
     got = o.render(nlines)
     o.close()
-    want = orc.run_ref(mode, rate, nlines, vfilter=filt, extra=extra)
-    assert got.size == want.size
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=filt, extra=extra))
 
 
 PASSTHRU_CASES = [
@@ -71,37 +119,30 @@ PASSTHRU_CASES = [
 
 
 @pytest.mark.parametrize("mode,rate,filt,extra,ext_lines", PASSTHRU_CASES)
-def test_passthru_alignment(built, tmp_path, mode, rate, filt, extra, ext_lines):
+def test_passthru_alignment(built, mode, rate, filt, extra, ext_lines):
     """ref _vid_passthru_process video.c:3517-3541: line alignment (the external stream's first
     line is spent on the filter's fill line), int16 wrap, whole lines only at its end."""
-    rng = np.random.default_rng(11)
     o = orc.Oracle(_conf(built, mode, filt, extra), rate)
-    W = o.width
-    ext = rng.integers(-32768, 32767, size=(ext_lines * W + W // 3, 2), dtype=np.int16)
+    ext = passthru_stream(o.width, ext_lines)
     o.open_test_source()
     o.set_passthru(ext)
     got = o.render(30)
     o.close()
-    fn = tmp_path / "ext.iq"
-    ext.tofile(fn)
-    want = orc.run_ref(mode, rate, 30, vfilter=filt, extra=tuple(extra) + ("--passthru", str(fn)))
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
-    plain = orc.run_ref(mode, rate, 30, vfilter=filt, extra=extra)
-    assert not np.array_equal(plain, want)
+    assert_reference(got, ref_key(mode, rate, 30, vfilter=filt, extra=tuple(extra) + ("--passthru",), source=f"passthru{ext_lines}"))
+    assert digest(got) != golden_ref()[ref_key(mode, rate, 30, vfilter=filt, extra=extra)]["sha256"]
 
 
-def wss_overlay(built, mode, rate, wss="16:9"):
-    """What the reference's WSS stage does to line 23 (wss.c:154-193): part of the line set to black, then the
-    bit waveform added. Recovered from the reference itself: unfiltered, no sound, no colour (the SECAM stage
-    runs after WSS and would filter it), with and without --wss."""
+def wss_overlay(built, mode, rate):
+    """What the reference's WSS stage (--wss 16:9) does to line 23 (wss.c:154-193): part of the line set to black,
+    then the bit waveform added. Recovered from the reference's own line 23 (I channel), unfiltered, no sound, no
+    colour (the SECAM stage runs after WSS and would filter it), without and with --wss."""
     conf = built.mode_config(mode, noaudio=True)
     t = built.Tables(conf, rate)
-    W, half = int(t.get("geometry")[0]), int(t.get("geometry")[1])
+    half = int(t.get("geometry")[1])
     black = int(t.get("levels")[1])
     t.close()
-    per = 2 if conf.output_type == 0 else 1
-    plain = orc.run_ref(mode, rate, 30, extra=("--noaudio", "--nocolour")).reshape(30, W, per)[22, :, 0].astype(np.int32)
-    with_wss = orc.run_ref(mode, rate, 30, extra=("--noaudio", "--nocolour", "--wss", wss)).reshape(30, W, per)[22, :, 0].astype(np.int32)
+    plain = golden_wss_lines()[f"{mode}_{rate}_plain"].astype(np.int32)
+    with_wss = golden_wss_lines()[f"{mode}_{rate}_wss"].astype(np.int32)
     blank_to = int(round(rate * 42.5e-6))
     base = plain.copy()
     base[half:blank_to] = black
@@ -120,29 +161,28 @@ def test_vbi_overlay_is_where_the_reference_puts_wss(built, mode, rate, filt, ex
     o.add_vbi_line(23, add, rep)
     got = o.render(700)
     o.close()
-    want = orc.run_ref(mode, rate, 700, vfilter=filt, extra=tuple(extra) + ("--wss", "16:9"))
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
+    assert_reference(got, ref_key(mode, rate, 700, vfilter=filt, extra=tuple(extra) + ("--wss", "16:9")))
 
 
 def test_oracle_equals_reference_on_random_input(built):
-    rng = np.random.default_rng(7)
     conf = built.mode_config("i", vfilter=True)
     o = orc.Oracle(conf, 16000000)
-    frames = rng.integers(0, 1 << 24, size=(2, o.active_lines, o.active_width), dtype=np.uint32)
-    audio = rng.integers(-32768, 32767, size=(30000, 2), dtype=np.int16)
+    frames, audio = random_source(7, o.active_lines, o.active_width)
     o.set_source(frames, audio)
     got = o.render(1400)
     o.close()
-    want = orc.run_ref("i", 16000000, 1400, vfilter=True, frames=frames, audio=audio, audio_block=4000)
-    assert np.array_equal(got, want)
+    assert_reference(got, ref_key("i", 16000000, 1400, vfilter=True, source="random7"))
 
 
-def test_unpatched_heap_differs_only_near_line_ends():
+def test_unpatched_heap_differs_only_near_line_ends(built):
     """The stock allocator lets the chroma FIR read past its buffer (SURVEY.md §8c): the
-    masked comparison - everything further than 32 samples from a line boundary - is exact."""
-    a = orc.run_ref("i", 16000000, 700, vfilter=True).reshape(700, 1024, 2)
-    b = orc.run_ref("i", 16000000, 700, vfilter=True, rawheap=True).reshape(700, 1024, 2)
-    assert np.array_equal(a[:, 32:-32], b[:, 32:-32])
+    masked comparison with that build - everything further than 32 samples from a line boundary - is exact."""
+    o = orc.Oracle(built.mode_config("i", vfilter=True), 16000000)
+    o.open_test_source()
+    got = o.render(700).reshape(700, 1024, 2)
+    o.close()
+    want = golden_ref()[ref_key("i", 16000000, 700, vfilter=True, rawheap=True)]
+    assert digest(got[:, 32:-32]) == want["masked_32_sha256"]
 
 
 # --pixelrate (SURVEY.md section 8f rank 4): raster at the pixel rate, the reference's polyphase resampler
@@ -170,9 +210,7 @@ def test_pixelrate_resampler_equals_reference(built, mode, rate, prate, nlines, 
     o.open_test_source()
     got = o.render(nlines)
     o.close()
-    want = orc.run_ref(mode, rate, nlines, vfilter=filt, extra=tuple(extra) + ("--pixelrate", str(prate)))
-    assert got.size == want.size
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=filt, extra=tuple(extra) + ("--pixelrate", str(prate))))
 
 
 def test_pixelrate_later_window_and_random_input(built):
@@ -182,35 +220,26 @@ def test_pixelrate_later_window_and_random_input(built):
     o.open_test_source()
     got = o.render(1700)[1400 * 2048:]
     o.close()
-    want = orc.run_ref("i", 16000000, 300, skip=1400, vfilter=True, extra=("--pixelrate", "13500000"))
-    assert np.array_equal(got, want)
-    rng = np.random.default_rng(5)
+    assert_reference(got, ref_key("i", 16000000, 300, skip=1400, vfilter=True, extra=("--pixelrate", "13500000")))
     o = orc.Oracle(conf, 16000000, 13500000)
-    frames = rng.integers(0, 1 << 24, size=(2, o.active_lines, o.active_width), dtype=np.uint32)
-    audio = rng.integers(-32768, 32767, size=(30000, 2), dtype=np.int16)
+    frames, audio = random_source(5, o.active_lines, o.active_width)
     o.set_source(frames, audio)
     got = o.render(900)
     o.close()
-    want = orc.run_ref("i", 16000000, 900, vfilter=True, frames=frames, audio=audio, audio_block=4000,
-                       extra=("--pixelrate", "13500000"))
-    assert np.array_equal(got, want)
+    assert_reference(got, ref_key("i", 16000000, 900, vfilter=True, extra=("--pixelrate", "13500000"), source="random5"))
 
 
-def test_pixelrate_with_passthru_and_wss(built, tmp_path):
+def test_pixelrate_with_passthru_and_wss(built):
     """Two fill lines in front of the stream (resampler + filter): the passthru stage spends two external
     lines on them; the VBI stages sit in front of the resampler."""
-    rng = np.random.default_rng(3)
     conf = built.mode_config("i", vfilter=True)
     o = orc.Oracle(conf, 16000000, 13500000)
-    ext = rng.integers(-32768, 32767, size=(40 * o.width + 100, 2), dtype=np.int16)
+    ext = passthru_stream(o.width, 40, seed=3, tail=100)
     o.open_test_source()
     o.set_passthru(ext)
     got = o.render(30)
     o.close()
-    fn = tmp_path / "ext.iq"
-    ext.tofile(fn)
-    want = orc.run_ref("i", 16000000, 30, vfilter=True, extra=("--pixelrate", "13500000", "--passthru", str(fn)))
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
+    assert_reference(got, ref_key("i", 16000000, 30, vfilter=True, extra=("--pixelrate", "13500000", "--passthru"), source="passthru40s3"))
 
     add, rep = wss_overlay(built, "pal", 13500000)               # the waveform at the pixel rate
     o = orc.Oracle(built.mode_config("pal"), 16000000, 13500000)
@@ -218,8 +247,7 @@ def test_pixelrate_with_passthru_and_wss(built, tmp_path):
     o.add_vbi_line(23, add, rep)
     got = o.render(100)
     o.close()
-    want = orc.run_ref("pal", 16000000, 100, extra=("--pixelrate", "13500000", "--wss", "16:9"))
-    assert np.array_equal(got, want), f"{np.count_nonzero(got != want)} values differ"
+    assert_reference(got, ref_key("pal", 16000000, 100, extra=("--pixelrate", "13500000", "--wss", "16:9")))
 
 
 def test_pixelrate_pairs_the_oracle_does_not_restate(built):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Device-resident throughput of every BASELINE.json config on one GPU (not the graded
-bench - that is bench.py, config 2). Prints one JSON line per config; used for
-profiles/*.md. Run on the GPU box: python tools/bench_configs.py"""
+bench - that is bench.py, config 2). Prints one JSON line per config.
+    python tools/bench_configs.py"""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

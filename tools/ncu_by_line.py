@@ -5,7 +5,7 @@
 
 Needs the product built with -lineinfo (it is) and nvdisasm/cuobjdump from the toolkit.
 Correlates `ncu --page source --csv` rows (in SASS order) with `nvdisasm -g` line markers
-of the sm_100a cubin embedded in hacktv_b200/libhacktv_b200.so."""
+of the sm_90a cubin embedded in hacktv_b200/libhacktv_b200.so."""
 import collections, csv, os, re, subprocess, sys, tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -15,7 +15,7 @@ topn = int(sys.argv[3]) if len(sys.argv) > 3 else 45
 
 with tempfile.TemporaryDirectory() as td:
     subprocess.run(["cuobjdump", "-xelf", "all", os.path.join(ROOT, "hacktv_b200", "libhacktv_b200.so")], cwd=td, capture_output=True)
-    cubin = [f for f in os.listdir(td) if "sm_100a" in f][0]
+    cubin = [f for f in os.listdir(td) if "sm_90a" in f][0]
     dis = subprocess.run(["nvdisasm", "-g", "-c", os.path.join(td, cubin)], capture_output=True, text=True).stdout.split("\n")
     # a report with several kernels: NCU_KERNEL=<base name> selects one (ncu --kernel-name)
     sel = ["--kernel-name", os.environ["NCU_KERNEL"]] if os.environ.get("NCU_KERNEL") else []

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The numbers profiles/r02_summary.md and bench.py quote from one `ncu --set full` report: selected raw metrics,
+"""Selected figures of one `ncu --set full` report: selected raw metrics,
 the warp-state sample breakdown, executed warp instructions by opcode.   tools/ncu_raw_summary.py <report> <samples>"""
 import collections, csv, re, subprocess, sys
 rep, samples = sys.argv[1], int(sys.argv[2])

@@ -1,6 +1,6 @@
 // Micro-benchmark: legacy mma.sync throughput on this GPU - IMMA m16n8k32 (s8), IMMA m16n8k16 (s8),
 // HMMA m16n8k16 (f16 -> f32, bf16 -> f32). Each warp keeps NCH independent accumulator chains.
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o tools/ubench_mma tools/ubench_mma.cu
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o tools/ubench_mma tools/ubench_mma.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,5 +1,5 @@
 // Micro-benchmark: issue throughput of IMAD, IDP.2A (dp2a), IADD3, FFMA on this GPU.
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o /tmp/ubench tools/ubench_pipes.cu
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o /tmp/ubench tools/ubench_pipes.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 template<int OP> __global__ void k(int *out, int n, int a0, int b0)
