@@ -2832,6 +2832,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			KL_ATTR(false, false); KL_ATTR(true, false); KL_ATTR(true, true);
 			#undef KL_ATTR
 			#undef KL_ATTR2
+			cudaFuncSetAttribute(k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem);
 		}
 	}
 	if(secam)
@@ -3204,6 +3205,10 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		#define KL_GO(VF, HQ) do { if(dp.W % MF_TILE == 0 && !d->kl_csat) KL_GO2(VF, HQ, true, false); \
 			else if(!d->kl_csat) KL_GO2(VF, HQ, false, false); else KL_GO2(VF, HQ, false, true); } while(0)
 		if(!dp.vf_type) KL_GO(false, false);
+		// ... and within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those sound stages
+		// and the width compiled in
+		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM)
+			k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
 		else if(dp.vf_type == 3) KL_GO(true, true);
 		else KL_GO(true, false);
 		#undef KL_GO

@@ -40,6 +40,26 @@ __device__ __forceinline__ int kl_acc15(int hh, int mid, int ll)
 }
 __device__ __forceinline__ int kl_fir_out(int hh, int mid, int ll) { return(sat16i(kl_acc15(hh, mid, ll))); }
 
+// SND: the sound carriers and post-modulation stages an instantiation has compiled in, as a mask of the flags below, or
+// -1 for the general form, which tests dp on every line. They are fixed for an encoder's life, so the host picks the
+// instantiation from dp (kl_snd_mask). Only the mask of the PAL systems with FM mono and NICAM on a VSB carrier has its
+// own instantiation, and only at W = 1024 (16 Msps), with the width compiled in too (WC); at 320 threads the fixed form
+// spills.
+#define KL_FM   1
+#define KL_AM   2
+#define KL_NIC  4
+#define KL_OFF  8
+#define KL_SWAP 16
+#define KL_CPX  32
+#define KL_SND_FM_NICAM (KL_FM | KL_NIC | KL_CPX)
+#define KL_HAS(SND, BIT, RT) ((SND) < 0 ? (RT) != 0 : ((SND) & (BIT)) != 0)
+
+static inline int kl_snd_mask(const htv_dparams_t &dp)
+{
+	return((dp.have_fm ? KL_FM : 0) | (dp.have_am ? KL_AM : 0) | (dp.have_nicam ? KL_NIC : 0) |
+		(dp.have_offset ? KL_OFF : 0) | (dp.swap_iq ? KL_SWAP : 0) | (dp.complex_out ? KL_CPX : 0));
+}
+
 // ---- sound carriers for the four samples of a lane (strided by 8) --------------------------------------------
 // Same arithmetic as sound_add<false> (ref video.c:3261-3450, nicam728.c:342-411); what differs is how a lane
 // finds its audio segment and NICAM symbol: all four samples lie in the 32-sample block b = xb >> 5, for which
@@ -48,11 +68,13 @@ __device__ __forceinline__ int kl_fir_out(int hh, int mid, int ll) { return(sat1
 // FM carrier: one sin/cos for the lane's first sample, the other three by rotating with the segment's
 // (cos, sin) of 8 angle steps - unless an audio-segment boundary or a renormalisation of the reference's
 // phasor (every 32 767 samples) falls between the lane's samples; then every sample gets its own.
+template<int SND>
 __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
 	const short *ntp, int xb, int (&oi)[4], int (&oq)[4])
 {
 	const int b = xb >> 5;
-	if(dp.have_fm || dp.have_am)
+	const bool fm = KL_HAS(SND, KL_FM, dp.have_fm), am = KL_HAS(SND, KL_AM, dp.have_am);
+	if(fm || am)
 	{
 		const int sg = la->fm_blk[b];
 		const int nb = la->seg_x[sg + 1];
@@ -62,7 +84,7 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 		// amplitude of the reference's Q31 phasor kk + 1 multiplications after a renormalisation
 		const float kf = (float) (kk + 1);
 		const bool mixed = (nb > xb && nb <= xb + 24) || kk + 25 > 32767;
-		if(dp.have_fm)
+		if(fm)
 		{
 			if(!mixed)
 			{
@@ -103,7 +125,7 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 				}
 			}
 		}
-		if(dp.have_am)
+		if(am)
 		{
 			unsigned long long phM = la->am_phase0 + dp.am_ang * (unsigned long long) (xb + 1);
 			const unsigned long long stM = dp.am_ang << 3;
@@ -124,7 +146,7 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 		}
 	}
 
-	if(dp.have_nicam)
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
 	{
 		int bi[4], bq[4];
 		if(!la->nic_generic)
@@ -180,17 +202,16 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 }
 
 // Mixers after the modulation (ref video.c:3466-3515), channel combiner, store - post_store for the strided layout
-template<bool FULL>
+template<bool FULL, int SND>
 __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
-	int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
+	int W, int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
 {
-	const int W = dp.W;
-	if(dp.swap_iq)
+	if(KL_HAS(SND, KL_SWAP, dp.swap_iq))
 	{
 		#pragma unroll
 		for(int j = 0; j < 4; j++) { const int t = oi[j]; oi[j] = oq[j]; oq[j] = t; }
 	}
-	if(dp.have_offset)
+	if(KL_HAS(SND, KL_OFF, dp.have_offset))
 	{
 		const long long m0 = la->m0;
 		const unsigned long long off0 = la->off_phase0;
@@ -220,7 +241,7 @@ __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const Dev
 		}
 	}
 	const size_t lbase = (size_t) row * (size_t) W;
-	if(dp.complex_out)
+	if(KL_HAS(SND, KL_CPX, dp.complex_out))
 	{
 		unsigned *o = reinterpret_cast<unsigned *>(out) + lbase + xb;
 		const unsigned *a = acc ? reinterpret_cast<const unsigned *>(acc) + lbase + xb : NULL;
@@ -266,13 +287,14 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 //
 // SRC: the composite lines are not rastered here but read from `src` (row q + 2 = relative line q, int16): SECAM, whose
 // chrominance chain (htv_secam.cuh) runs between the raster and the modulator. R1b / R2 fold away, the rest is the same.
-template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false>
+// WC: the line width compiled in (0: dp.W), so that the shared-memory row and plane offsets become immediates
+template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap,
 	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
-	const int W = dp.W;
+	const int W = WC ? WC : dp.W;
 	const int RB = kl_row_bytes(W), UB = kl_uv_bytes(W);
 	// descriptors x2 | [row 0..2][hi, lo] composite planes | [u hi, u lo, v hi, v lo] | FIR taps | chroma taps | NICAM pulse
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
@@ -295,7 +317,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	if(VF) for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
 	if(dt.chroma_atab) for(int i = tid; i < 64; i += blockDim.x) ctab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.chroma_atab) + i);
 	for(int i = tid; i < ((VF ? 6 * RB : 0) + 4 * UB) / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
-	if(dp.have_nicam)
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
 	{
 		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
 		int4 *dst = reinterpret_cast<int4 *>(ntp);
@@ -541,8 +563,8 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		if(FULL || xb < W)
 		{
 			const LineA2 *la = sla + (mrow & 1);
-			kl_sound(dp, dt, la, ntp, xb, oi, oq);
-			kl_post_store<FULL>(dp, dt, la, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
+			kl_sound<SND>(dp, dt, la, ntp, xb, oi, oq);
+			kl_post_store<FULL, SND>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
 		}
 	}
 	#undef KL_R1A
