@@ -147,6 +147,7 @@ def lib() -> C.CDLL:
         getattr(L, f).restype = C.c_int; getattr(L, f).argtypes = [vp]
     L.htv_lines_rendered.restype = i64; L.htv_lines_rendered.argtypes = [vp]
     L.htv_kernel_launches.restype = C.c_uint64; L.htv_kernel_launches.argtypes = [vp]
+    L.htv_line_kernel.restype = C.c_char_p; L.htv_line_kernel.argtypes = [vp]
     L.htv_set_kernel_timing.restype = None; L.htv_set_kernel_timing.argtypes = [vp, C.c_int]
     L.htv_last_line_kernel_ms.restype = C.c_float; L.htv_last_line_kernel_ms.argtypes = [vp]
     L.htv_last_line_kernel_lines.restype = C.c_int; L.htv_last_line_kernel_lines.argtypes = [vp]
@@ -406,6 +407,11 @@ class Encoder:
     @property
     def kernel_launches(self) -> int:
         return int(self._L.htv_kernel_launches(self._h))
+
+    @property
+    def line_kernel(self) -> str:
+        """The line kernel(s) the most recent render launched, with their template arguments (htv_line_kernel)."""
+        return self._L.htv_line_kernel(self._h).decode()
 
     def set_kernel_timing(self, on: bool):
         self._L.htv_set_kernel_timing(self._h, int(on))

@@ -230,6 +230,7 @@ int htv_is_complex(const htv_t *s) { return(s->complex); }
 int htv_bytes_per_sample(const htv_t *s) { return(s->bps); }
 int64_t htv_lines_rendered(const htv_t *s) { return(s->next_line); }
 uint64_t htv_kernel_launches(const htv_t *s) { return(htv_dev_launches(s->dev)); }
+const char *htv_line_kernel(const htv_t *s) { return(htv_dev_line_kernel(s->dev)); }
 void htv_set_kernel_timing(htv_t *s, int on) { htv_dev_set_timing(s->dev, on); }
 float htv_last_line_kernel_ms(htv_t *s) { return(htv_dev_last_line_ms(s->dev)); }
 int htv_last_line_kernel_lines(const htv_t *s) { return(htv_dev_last_line_count(s->dev)); }

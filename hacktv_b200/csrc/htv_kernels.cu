@@ -191,6 +191,8 @@ struct htv_dev_t {
 	int desc_cap;
 	// the fused line kernel (htv_line.cuh): PAL / NTSC / mono, AM or VSB, no resampler
 	int use_line, kl_threads, kl_ctas, kl_csat;
+	int kl_general;                   // HTV_KL=general: never the instantiation with the sound stages and width compiled in
+	char kname[192];                  // the line kernel(s) the last render launched, with their template arguments (htv_line_kernel)
 	int sec_line;                     // SECAM: the modulator is the fused line kernel in its SRC form (composite rows from d_comp)
 	size_t ks_smem;                   // ... and the raster is k_sec_raster (0: k_raster_secam)
 	size_t kl_smem;
@@ -2818,8 +2820,12 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			d->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (dp.vf_type ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 +
 				sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
 			d->use_line = 1;
+			// HTV_KL=general: the general instantiation where the one with the sound stages compiled in would run (A/B, tests)
+			d->kl_general = getenv("HTV_KL") && !strcmp(getenv("HTV_KL"), "general");
 			{
-				// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768 (Gaussian taps: always)
+				// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768. The Gaussian taps are
+				// rounded one by one, so at about 1 % of sample rates they sum to 32769 .. 32771 (17.734475, 20.05 Msps: 32769),
+				// and those rates run the CSAT form
 				long long sum = 0;
 				for(int i = 0; i < dp.chroma_ntaps; i++) sum += dp.chroma_taps[i] < 0 ? -dp.chroma_taps[i] : dp.chroma_taps[i];
 				d->kl_csat = sum > 32768;
@@ -3129,6 +3135,13 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	return(HTV_OK);
 }
 
+// The instantiation of the fused line kernel a launch uses, every template argument spelled out (htv_line_kernel); written
+// next to each launch, so that a change to the selection shows up in the name
+static void kl_name(char *s, size_t n, bool vf, bool hq, bool full, bool csat, int maxt, bool src, int snd, int wc)
+{
+	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d>", vf, hq, full, csat, maxt, src, snd, wc);
+}
+
 extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int16_t *d_out,
 	const int16_t *d_acc, int acc_lines, void *stream)
 {
@@ -3197,22 +3210,29 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		if(run < 4) run = 4;
 		const int grid = (nlines + run - 1) / run;
 		if(d->timing) cudaEventRecord(d->ev0, st);
+		#define KL_GO3(VF, HQ, FU, CS, T, B) do { \
+			kl_name(d->kname, sizeof(d->kname), VF, HQ, FU, CS, T, false, -1, 0); \
+			k_line<VF, HQ, FU, CS, T, B><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); } while(0)
 		#define KL_GO2(VF, HQ, FU, CS) do { \
-			if(d->kl_threads <= 256) k_line<VF, HQ, FU, CS, 256, KL_B256><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); \
-			else if(d->kl_threads <= 320) k_line<VF, HQ, FU, CS, 320, KL_B320><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); \
-			else k_line<VF, HQ, FU, CS, 384, KL_B384><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); } while(0)
+			if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, CS, 256, KL_B256); \
+			else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, CS, 320, KL_B320); \
+			else KL_GO3(VF, HQ, FU, CS, 384, KL_B384); } while(0)
 		// the common case (128 | W, a chroma filter that cannot overflow) gets its own instantiation; everything else the general one
 		#define KL_GO(VF, HQ) do { if(dp.W % MF_TILE == 0 && !d->kl_csat) KL_GO2(VF, HQ, true, false); \
 			else if(!d->kl_csat) KL_GO2(VF, HQ, false, false); else KL_GO2(VF, HQ, false, true); } while(0)
 		if(!dp.vf_type) KL_GO(false, false);
 		// ... and within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those sound stages
 		// and the width compiled in
-		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM)
+		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !d->kl_general)
+		{
+			kl_name(d->kname, sizeof(d->kname), true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024);
 			k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
+		}
 		else if(dp.vf_type == 3) KL_GO(true, true);
 		else KL_GO(true, false);
 		#undef KL_GO
 		#undef KL_GO2
+		#undef KL_GO3
 		CK(cudaEventRecord(d->ev_kl[buf], st));
 		d->launches += 4;
 		d->last_mod_lines = nlines;
@@ -3254,6 +3274,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * d->dp.W * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
+		char rname[64], mname[128];                   // raster and modulator kernels of this sub-batch (htv_line_kernel)
 		if(d->dp.colour_mode == HTV_SECAM)
 		{
 			// rows 0 .. n+2 <-> lines first-2 .. first+n; the chain covers rows 0 .. n+1
@@ -3267,15 +3288,23 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				if(run < 4) run = 4;
 				const int grid = (nr + run - 1) / run;
 				const bool full = d->dp.W % MF_TILE == 0;
+				#define KS_GO2(FU, T, B) do { \
+					snprintf(rname, sizeof(rname), "k_sec_raster<FULL=%d,MAXT=%d>", FU, T); \
+					k_sec_raster<FU, T, B><<<grid, d->kl_threads, d->ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec); } while(0)
 				#define KS_GO(FU) do { \
-					if(d->kl_threads <= 256) k_sec_raster<FU, 256, KL_B256><<<grid, d->kl_threads, d->ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec); \
-					else if(d->kl_threads <= 320) k_sec_raster<FU, 320, KL_B320><<<grid, d->kl_threads, d->ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec); \
-					else k_sec_raster<FU, 384, KL_B384><<<grid, d->kl_threads, d->ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec); } while(0)
+					if(d->kl_threads <= 256) KS_GO2(FU, 256, KL_B256); \
+					else if(d->kl_threads <= 320) KS_GO2(FU, 320, KL_B320); \
+					else KS_GO2(FU, 384, KL_B384); } while(0)
 				if(full) KS_GO(true); else KS_GO(false);
 				#undef KS_GO
+				#undef KS_GO2
 				d->launches++;
 			}
-			else k_raster_secam<<<n + 3, d->line_threads, d->raster_smem, st>>>(d->dp, d->dt, lr, d->d_comp, d->sec);
+			else
+			{
+				snprintf(rname, sizeof(rname), "k_raster_secam");
+				k_raster_secam<<<n + 3, d->line_threads, d->raster_smem, st>>>(d->dp, d->dt, lr, d->d_comp, d->sec);
+			}
 			// the chain (htv_secam.cuh): pass 0 over every line, the predictor, then refinement passes until no line's
 			// outgoing state changes - at that fixed point every line was computed from its true predecessor state =
 			// the sequential result. The loop needs the change count on the host, so SECAM launches synchronise.
@@ -3339,6 +3368,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		else
 		{
 			// raster lines done-1 .. done+n (descriptor index = line - (line0 - 1))
+			snprintf(rname, sizeof(rname), "k_raster");
 			k_raster<<<n + 2, d->line_threads, d->raster_smem, st>>>(d->dp, d->dt, ld.r + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, d->plane_pitch);
 			d->launches++;
 		}
@@ -3360,6 +3390,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			else { fprintf(stderr, "hacktv_b200: unsupported FM pre-emphasis length %d\n", dp.fmv_ntaps); return(HTV_ERROR); }
 			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, rows);
 			k_fmv_mod<<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
+			snprintf(mname, sizeof(mname), "k_fmv_base<%d> + k_fmv_scan + k_fmv_mod", dp.fmv_ntaps);
 			d->launches += 2;
 		}
 		else if(d->sec_line)
@@ -3369,31 +3400,36 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			int run = (n + d->kl_ctas - 1) / d->kl_ctas;
 			if(run < 4) run = 4;
 			const int grid = (n + run - 1) / run;
+			#define KL_GO3(VF, HQ, FU, T, B) do { \
+				kl_name(mname, sizeof(mname), VF, HQ, FU, false, T, true, -1, 0); \
+				k_line<VF, HQ, FU, false, T, B, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); } while(0)
 			#define KL_GO2(VF, HQ, FU) do { \
-				if(d->kl_threads <= 256) k_line<VF, HQ, FU, false, 256, KL_B256, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); \
-				else if(d->kl_threads <= 320) k_line<VF, HQ, FU, false, 320, KL_B320, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); \
-				else k_line<VF, HQ, FU, false, 384, KL_B384, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); } while(0)
+				if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, 256, KL_B256); \
+				else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, 320, KL_B320); \
+				else KL_GO3(VF, HQ, FU, 384, KL_B384); } while(0)
 			#define KL_GO(VF, HQ) do { if(dp.W % MF_TILE == 0) KL_GO2(VF, HQ, true); else KL_GO2(VF, HQ, false); } while(0)
 			if(!dp.vf_type) KL_GO(false, false);
 			else if(dp.vf_type == 3) KL_GO(true, true);
 			else KL_GO(true, false);
 			#undef KL_GO
 			#undef KL_GO2
+			#undef KL_GO3
 		}
 		else if(d->d_planes)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows);
-			else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows);
+			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_mma<256,4>"); k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); }
+			else { snprintf(mname, sizeof(mname), "k_mod_mma<384,2>"); k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); }
 		}
 		else if(d->d_comp32)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows);
-			else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows);
+			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_tma<256,4>"); k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); }
+			else { snprintf(mname, sizeof(mname), "k_mod_tma<384,2>"); k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); }
 		}
-		else if(d->line_threads <= 256) k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows);
-		else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows);
+		else if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod<256,4>"); k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); }
+		else { snprintf(mname, sizeof(mname), "k_mod<384,2>"); k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); }
+		snprintf(d->kname, sizeof(d->kname), "%s + %s", rname, mname);
 		d->launches++;
 		if(last) d->last_mod_lines = n;
 	}
@@ -3520,6 +3556,8 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 		else if(d->line_threads <= 256) k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows);
 		else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows);
 		d->launches++;
+		snprintf(d->kname, sizeof(d->kname), "k_raster + k_resample + %s<%d,%d>", d->d_planes ? "k_mod_mma" : d->d_comp32 ? "k_mod_tma" : "k_mod",
+			d->line_threads <= 256 ? 256 : 384, d->line_threads <= 256 ? 4 : 2);
 		if(last) d->last_mod_lines = n;
 	}
 	if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
@@ -3626,6 +3664,7 @@ extern "C" void *htv_dev_alloc_pinned(size_t bytes)
 extern "C" void htv_dev_free_pinned(void *p) { if(p) cudaFreeHost(p); }
 
 extern "C" uint64_t htv_dev_launches(const htv_dev_t *d) { return(d->launches); }
+extern "C" const char *htv_dev_line_kernel(const htv_dev_t *d) { return(d->kname); }
 extern "C" void htv_dev_set_timing(htv_dev_t *d, int on) { d->timing = on; }
 
 extern "C" int htv_dev_last_line_count(const htv_dev_t *d) { return(d->last_mod_lines); }

@@ -293,6 +293,11 @@ extern int htv_bytes_per_sample(const htv_t *s);   /* 4 complex, 2 real */
 extern int64_t htv_lines_rendered(const htv_t *s);
 /* Kernel launches issued by this encoder since htv_init (for bench accounting) */
 extern uint64_t htv_kernel_launches(const htv_t *s);
+/* The line kernel(s) the most recent render launched, with their template arguments, e.g.
+ * "k_line<VF=1,HQ=1,FULL=0,CSAT=1,MAXT=384,SRC=0,SND=-1,WC=0>", or for SECAM
+ * "k_sec_raster<FULL=1,MAXT=384> + k_line<...,SRC=1,...>"; "" before the first render. Read-only diagnostic:
+ * the string belongs to the encoder and changes with the next render. */
+extern const char *htv_line_kernel(const htv_t *s);
 /* Duration of the dominant kernel's (k_mod) most recent launch, measured with CUDA
  * events on the stream it ran on (0 if timing is off), and the scan lines that launch covered. */
 extern void htv_set_kernel_timing(htv_t *s, int on);

@@ -57,6 +57,22 @@ CASES = [
 ]
 
 
+def _line_width_cases():
+    """Every mode, rate and option set the line kernel is held at by test_gpu_zz_line_widths.py, with the mode's sound
+    and the lines it renders: the oracle those tests compare with is the reference there too."""
+    from test_gpu_zz_line_widths import MATRIX
+    out = []
+    for mode, rate, kw, _, _ in MATRIX:
+        extra = tuple(f"--{k}" for k in ("nocolour", "nonicam") if kw.get(k))
+        case = (mode, rate, 290 if mode in ("m", "ntsc") else 340, bool(kw.get("vfilter")), extra)
+        if case not in CASES and case not in out:
+            out.append(case)
+    return out
+
+
+CASES += _line_width_cases()
+
+
 def ref_key(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", rawheap=False):
     """Names one reference run in golden_ref.json: its command line, with the input it was given instead of file
     names (`source`: the built-in test source, or which seeded random input / passthru stream)."""

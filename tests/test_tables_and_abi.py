@@ -168,3 +168,60 @@ def test_pixelrate_pairs_that_are_refused(built):
     t = built.Tables(built.mode_config("i"), 16000000, 16000000)             # no resampler at all
     assert t.get("rs_taps") is None
     t.close()
+
+
+def _line_kernel_from_tables(H, mode, rate, kw):
+    """The line kernel htv_dev_create / htv_dev_render_lines select for an encoder, from its tables alone, with the
+    facts the selection rests on: W, its tiles of 128 samples, the last tile's width and the chroma taps' sum."""
+    conf = H.mode_config(mode, **kw)
+    t = H.Tables(conf, rate)
+    W = int(t.get("geometry")[0])
+    ct = t.get("chroma_taps")
+    vf, hq = int(t.get("vsb_itaps") is not None), int(t.get("vsb_qtaps") is not None)
+    t.close()
+    tiles = -(-W // 128)
+    maxt = 256 if tiles <= 8 else 320 if tiles <= 10 else 384
+    tap_sum = 0 if ct is None else int(np.abs(ct).sum())
+    if conf.colour_mode == 3:                                   # SECAM: no chroma low-pass in the line kernel
+        full = int(W % 128 == 0)
+        return W, tiles, W % 128, tap_sum, f"k_sec_raster<FULL={full},MAXT={maxt}> + " + \
+            f"k_line<VF={vf},HQ={hq},FULL={full},CSAT=0,MAXT={maxt},SRC=1,SND=-1,WC=0>"
+    assert conf.colour_mode == 0 or 3 <= len(ct) <= 17, "the chroma low-pass does not fit the line kernel"
+    csat = int(tap_sum > 32768)
+    full = int(W % 128 == 0 and not csat)
+    return W, tiles, W % 128, tap_sum, f"k_line<VF={vf},HQ={hq},FULL={full},CSAT={csat},MAXT={maxt},SRC=0,SND=-1,WC=0>"
+
+
+def test_line_width_matrix_selects_what_each_case_is_for(built):
+    """The GPU line-width matrix (test_gpu_zz_line_widths.py) without a GPU: every case's W, tile count, last tile and
+    chroma saturation condition are what the tables give, and the instantiation it names is the one they select."""
+    from test_gpu_zz_line_widths import MATRIX
+    for mode, rate, kw, W, kernel in MATRIX:
+        w, tiles, residue, tap_sum, sel = _line_kernel_from_tables(built, mode, rate, kw)
+        what = f"{mode} {rate} {kw}"
+        assert w == W, (what, w)
+        assert f"MAXT={256 if tiles <= 8 else 320 if tiles <= 10 else 384}" in kernel and tiles <= 12, (what, tiles)
+        assert ("CSAT=1" in kernel) == (tap_sum > 32768), (what, tap_sum)
+        assert ("FULL=1" in kernel) == (residue == 0 and tap_sum <= 32768), (what, residue)
+        assert sel == kernel, (what, sel)
+
+
+def test_line_width_matrix_covers_every_instantiation(built):
+    """Together the matrix and the compiled-in sound form run every k_line and k_sec_raster instantiation
+    htv_dev_create sets up: VF / HQ x {FULL, partial, CSAT} x MAXT, the SECAM SRC form's VF / HQ x FULL x MAXT and its
+    raster's FULL x MAXT (SECAM has no chroma low-pass here, so no CSAT form), and the 16 Msps form with PAL's sound
+    stages compiled in. No instantiation is unreachable from the modes and rates the tables accept."""
+    from test_gpu_zz_line_widths import FIXED, MATRIX
+    kl = "k_line<VF={},HQ={},FULL={},CSAT={},MAXT={},SRC={},SND=-1,WC=0>"
+    want = {FIXED}
+    for maxt in (256, 320, 384):
+        for vf, hq in ((0, 0), (1, 0), (1, 1)):
+            for full, csat in ((1, 0), (0, 0), (0, 1)):
+                want.add(kl.format(vf, hq, full, csat, maxt, 0))
+            for full in (0, 1):
+                want.add(kl.format(vf, hq, full, 0, maxt, 1))
+        for full in (0, 1):
+            want.add(f"k_sec_raster<FULL={full},MAXT={maxt}>")
+    ran = {FIXED} | {part for c in MATRIX for part in c[4].split(" + ")}
+    assert not want - ran, sorted(want - ran)
+    assert not ran - want, sorted(ran - want)
