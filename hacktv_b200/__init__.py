@@ -76,6 +76,13 @@ _READ_AUDIO = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(
 _PASSTHRU_READ = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)
 
 
+class SecamChain(C.Structure):
+    """htv_secam_chain_t"""
+    _fields_ = [(n, C.c_int64) for n in ("launches", "passes", "final_odd", "final_even", "recomputed", "listed_warp",
+                                         "listed_thread", "repredict_odd", "repredict_even")] + \
+               [("passes_max", C.c_int32), ("list_max", C.c_int32)]
+
+
 class VbiLine(C.Structure):
     """htv_vbi_line_t"""
     _fields_ = [("line", C.c_int), ("replace_from", C.c_int), ("replace_to", C.c_int), ("replace_value", C.c_int),
@@ -148,6 +155,7 @@ def lib() -> C.CDLL:
     L.htv_lines_rendered.restype = i64; L.htv_lines_rendered.argtypes = [vp]
     L.htv_kernel_launches.restype = C.c_uint64; L.htv_kernel_launches.argtypes = [vp]
     L.htv_line_kernel.restype = C.c_char_p; L.htv_line_kernel.argtypes = [vp]
+    L.htv_secam_chain.restype = C.c_int; L.htv_secam_chain.argtypes = [vp, C.POINTER(SecamChain)]
     L.htv_set_kernel_timing.restype = None; L.htv_set_kernel_timing.argtypes = [vp, C.c_int]
     L.htv_last_line_kernel_ms.restype = C.c_float; L.htv_last_line_kernel_ms.argtypes = [vp]
     L.htv_last_line_kernel_lines.restype = C.c_int; L.htv_last_line_kernel_lines.argtypes = [vp]
@@ -412,6 +420,16 @@ class Encoder:
     def line_kernel(self) -> str:
         """The line kernel(s) the most recent render launched, with their template arguments (htv_line_kernel)."""
         return self._L.htv_line_kernel(self._h).decode()
+
+    @property
+    def secam_chain(self) -> dict:
+        """What the SECAM chain did since the encoder was created, summed over its launches (htv_secam_chain): launches,
+        passes, passes_max, final_odd / final_even, recomputed, listed_warp / listed_thread, list_max,
+        repredict_odd / repredict_even. All zero for other colour modes."""
+        c = SecamChain()
+        if self._L.htv_secam_chain(self._h, C.byref(c)) != HTV_OK:
+            raise RuntimeError("htv_secam_chain failed")
+        return {name: int(getattr(c, name)) for name, _ in SecamChain._fields_}
 
     def set_kernel_timing(self, on: bool):
         self._L.htv_set_kernel_timing(self._h, int(on))

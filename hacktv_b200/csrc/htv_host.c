@@ -231,6 +231,12 @@ int htv_bytes_per_sample(const htv_t *s) { return(s->bps); }
 int64_t htv_lines_rendered(const htv_t *s) { return(s->next_line); }
 uint64_t htv_kernel_launches(const htv_t *s) { return(htv_dev_launches(s->dev)); }
 const char *htv_line_kernel(const htv_t *s) { return(htv_dev_line_kernel(s->dev)); }
+int htv_secam_chain(const htv_t *s, htv_secam_chain_t *out)
+{
+	if(!s || !out) return(HTV_ERROR);
+	htv_dev_secam_chain(s->dev, out);
+	return(HTV_OK);
+}
 void htv_set_kernel_timing(htv_t *s, int on) { htv_dev_set_timing(s->dev, on); }
 float htv_last_line_kernel_ms(htv_t *s) { return(htv_dev_last_line_ms(s->dev)); }
 int htv_last_line_kernel_lines(const htv_t *s) { return(htv_dev_last_line_count(s->dev)); }

@@ -167,6 +167,7 @@ extern void *htv_dev_alloc_pinned(size_t bytes);
 extern void htv_dev_free_pinned(void *p);
 extern uint64_t htv_dev_launches(const htv_dev_t *d);
 extern const char *htv_dev_line_kernel(const htv_dev_t *d);
+extern void htv_dev_secam_chain(const htv_dev_t *d, htv_secam_chain_t *out);
 extern void htv_dev_set_timing(htv_dev_t *d, int on);
 extern float htv_dev_last_line_ms(htv_dev_t *d);
 extern int htv_dev_last_line_count(const htv_dev_t *d);

@@ -22,6 +22,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
+#include <limits.h>
 #include "htv_internal.h"
 #include "htv_mma_fir.h"
 #include "htv_resample.h"
@@ -197,7 +198,9 @@ struct htv_dev_t {
 	size_t ks_smem;                   // ... and the raster is k_sec_raster (0: k_raster_secam)
 	size_t kl_smem;
 	SecScratch sec;                   // SECAM scratch (same sub-batch rows as d_comp)
-	int sec_passes;
+	// the SECAM chain's switches (HTV_SEC, sec_knobs) and what it did since the encoder was created (htv_secam_chain)
+	int sec_passes, sec_pred, sec_many, sec_repredict, sec_repredict_min, sec_sub;
+	htv_secam_chain_t sec_stats;
 	int *d_comp32;                    // int32 composite scratch for the TMA-fed modulator (4 | W, not SECAM)
 	uint8_t *d_planes;                // high / low byte planes of the composite stream for k_mod_mma (32 | W, video filter on)
 	size_t plane_stride, modm_smem;
@@ -2545,6 +2548,55 @@ extern "C" int htv_dev_count(void)
 
 extern "C" size_t htv_dev_audio_ring_pairs(void) { return(RA); }
 
+// HTV_SEC: test and A/B switches of the SECAM chain (DESIGN §6), comma-separated key=value pairs read when an encoder is
+// created. Unset, every value is the default below. An unknown key or a bad value fails the encoder: a typo must not
+// quietly run the default path.
+static bool sec_knobs(htv_dev_t *d, char *err, size_t errlen)
+{
+	d->sec_many = SEC_LIST_MANY; d->sec_pred = SEC_PRED; d->sec_repredict = 2; d->sec_repredict_min = 64;
+	d->sec_sub = 0; d->sec_passes = 64;
+	const char *env = getenv("HTV_SEC");
+	if(!env) return(true);
+	char buf[256];
+	if(strlen(env) >= sizeof(buf)) { snprintf(err, errlen, "HTV_SEC is longer than %d characters", (int) sizeof(buf) - 1); return(false); }
+	strcpy(buf, env);
+	char *save = NULL;
+	for(char *kv = strtok_r(buf, ",", &save); kv; kv = strtok_r(NULL, ",", &save))
+	{
+		char *v = strchr(kv, '=');
+		if(!v) { snprintf(err, errlen, "HTV_SEC: '%s' is not key=value", kv); return(false); }
+		*v++ = 0;
+		if(!strcmp(kv, "list"))
+		{
+			// the list kernel: by length (auto), always one warp per line, always one thread per line
+			if(!strcmp(v, "auto")) d->sec_many = SEC_LIST_MANY;
+			else if(!strcmp(v, "warp")) d->sec_many = INT_MAX;
+			else if(!strcmp(v, "thread")) d->sec_many = -1;
+			else { snprintf(err, errlen, "HTV_SEC: list=%s is not auto, warp or thread", v); return(false); }
+			continue;
+		}
+		const struct { const char *key; int *dst; long lo, hi; } num[] = {
+			{ "pred", &d->sec_pred, 0, 64 },                       // predictor iterations
+			{ "repredict", &d->sec_repredict, 0, 64 },             // re-predictions per launch
+			{ "repredict_min", &d->sec_repredict_min, -1, INT_MAX },  // listed lines above which one fires (-1: any change)
+			{ "sub", &d->sec_sub, 64, INT_MAX },                   // lines per chain launch (at most the default)
+			{ "passes", &d->sec_passes, 1, 1024 },                 // refinement passes before HTV_ERROR
+		};
+		int k = 0;
+		while(k < (int) (sizeof(num) / sizeof(num[0])) && strcmp(kv, num[k].key)) k++;
+		if(k == (int) (sizeof(num) / sizeof(num[0]))) { snprintf(err, errlen, "HTV_SEC: unknown key '%s'", kv); return(false); }
+		char *end = NULL;
+		const long x = strtol(v, &end, 10);
+		if(!*v || *end || x < num[k].lo || x > num[k].hi)
+		{
+			snprintf(err, errlen, "HTV_SEC: %s=%s is not an integer in [%ld, %ld]", kv, v, num[k].lo, num[k].hi);
+			return(false);
+		}
+		*num[k].dst = (int) x;
+	}
+	return(true);
+}
+
 extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame_slots, int device, char *err, size_t errlen)
 {
 	int n = 0;
@@ -2565,6 +2617,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	if(!d) { snprintf(err, errlen, "out of memory"); return(NULL); }
 	d->device = device;
 	d->dp = t->dp;
+	if(!sec_knobs(d, err, errlen)) { free(d); return(NULL); }
 	const htv_dparams_t &dp = d->dp;
 	DevTables &dt = d->dt;
 
@@ -2663,6 +2716,17 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	// SECAM: the cross-line chain is latency bound per launch, so one launch should cover the whole call
 	d->sub_lines = ((secam ? 160 : 16) * 1024 * 1024) / (W * 2);
 	if(d->sub_lines < 64) d->sub_lines = 64;
+	if(secam && d->sec_sub)
+	{
+		// HTV_SEC=sub=...: shorter chain launches, so that a call crosses launch boundaries (tests)
+		if(d->sec_sub > d->sub_lines)
+		{
+			snprintf(err, errlen, "HTV_SEC: sub=%d is more than the %d lines of one launch", d->sec_sub, d->sub_lines);
+			htv_dev_destroy(d);
+			return(NULL);
+		}
+		d->sub_lines = d->sec_sub;
+	}
 	if(cudaMalloc((void **) &d->d_comp, sizeof(int16_t) * ((size_t) d->sub_lines + 3) * W + 256) != cudaSuccess)
 	{
 		snprintf(err, errlen, "device allocation failed");
@@ -2870,7 +2934,6 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		d->sec.iyc = (double *) dev_zero(d, sizeof(double) * ((size_t) W / SEC_IYC + 2) * rows);
 		d->sec.chk = (SecChk *) dev_zero(d, sizeof(SecChk) * rows);
 		d->sec.list = (int *) dev_zero(d, sizeof(int) * rows);
-		d->sec_passes = 64;
 		if(!d->sec.cbT || !d->sec.flags || !d->sec.yT || !d->sec.phT || !d->sec.iyc || !d->sec.chk || !d->sec.list || !d->sec.outc)
 		{
 			snprintf(err, errlen, "device allocation failed");
@@ -3312,7 +3375,9 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			cudaEvent_t dbg0 = NULL, dbg1 = NULL;
 			const bool dbg = getenv("HTV_DEBUG") != NULL;
 			if(dbg) { cudaEventCreate(&dbg0); cudaEventCreate(&dbg1); cudaEventRecord(dbg0, st); }
-			int pass = 0, changed = 1, repredict = 2;
+			int pass = 0, changed = 1, repredict = d->sec_repredict;
+			htv_secam_chain_t &cs = d->sec_stats;
+			cs.launches++;
 			for(; pass <= d->sec_passes && changed; pass++)
 			{
 				int fl[4];
@@ -3321,40 +3386,48 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				{
 					k_sec_pass0<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, nch);
 					// propose the states pass 1 starts from (see k_sec_predict); st[0] takes them over
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch);
+					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, d->sec_pred);
 					cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 					d->launches += 2;
 					continue;
 				}
 				k_sec_refine<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, pass);
-				k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, lr, d->sec, pass);
-				k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, pass);
+				k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, lr, d->sec, pass, d->sec_many);
+				k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, pass, d->sec_many);
 				d->launches += 3;
 				CK(cudaMemcpyAsync(fl, d->sec.flags, sizeof(fl), cudaMemcpyDeviceToHost, st));
 				CK(cudaStreamSynchronize(st));
 				changed = fl[0];
+				// what the chain did, from the counts this pass copies back anyway
+				cs.passes++;
+				cs.recomputed += fl[2];
+				if(fl[3] > d->sec_many) cs.listed_thread += fl[3]; else cs.listed_warp += fl[3];
+				if(fl[3] > cs.list_max) cs.list_max = fl[3];
 				if(dbg)
 				{
 					float ms = 0;
 					cudaEventRecord(dbg1, st); cudaEventSynchronize(dbg1); cudaEventElapsedTime(&ms, dbg0, dbg1);
 					fprintf(stderr, "secam pass %d: recomputed %d (FM in full: %d), output changed %d, cumulative %.3f ms\n", pass, fl[2], fl[3], fl[0], ms);
 				}
-				if(changed && fl[3] > 64 && repredict > 0)
+				if(changed && fl[3] > d->sec_repredict_min && repredict > 0)
 				{
 					// many lines had their FM recurrence re-run: their A, B moved, and plain iteration would carry that down
 					// the lines at 3x per pass - propose again from the new checkpoints (the pass's outputs go to st[0] first)
 					repredict--;
+					if(pass & 1) cs.repredict_odd++; else cs.repredict_even++;
 					if(pass & 1) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch);
+					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, d->sec_pred);
 					if(!(pass & 1)) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 					d->launches++;
 				}
 			}
+			if(pass - 1 > cs.passes_max) cs.passes_max = pass - 1;
 			if(changed)
 			{
 				fprintf(stderr, "hacktv_b200: SECAM cross-line state did not converge in %d passes\n", d->sec_passes);
 				return(HTV_ERROR);
 			}
+			if((pass - 1) & 1) cs.final_odd++; else cs.final_even++;
 			k_sec_carry<<<1, 32, 0, st>>>(lr, d->sec, n - 1, pass - 1);
 			k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, lr, d->sec, d->d_comp, nch);
 			d->launches += 2;
@@ -3665,6 +3738,7 @@ extern "C" void htv_dev_free_pinned(void *p) { if(p) cudaFreeHost(p); }
 
 extern "C" uint64_t htv_dev_launches(const htv_dev_t *d) { return(d->launches); }
 extern "C" const char *htv_dev_line_kernel(const htv_dev_t *d) { return(d->kname); }
+extern "C" void htv_dev_secam_chain(const htv_dev_t *d, htv_secam_chain_t *out) { *out = d->sec_stats; }
 extern "C" void htv_dev_set_timing(htv_dev_t *d, int on) { d->timing = on; }
 
 extern "C" int htv_dev_last_line_count(const htv_dev_t *d) { return(d->last_mod_lines); }

@@ -298,12 +298,14 @@ k_sec_pass0(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const 
 // incoming A, B in sec_tail's handful of steps. A CTA keeps the tail inputs of its rows in registers and iterates
 // state[c] <- tail(c, state[c - 1]) SEC_PRED times through shared memory (the rows above the CTA's own are a halo that
 // starts from pass 0's outputs), so pass 1 starts from states that are right to 3^-SEC_PRED. It only proposes states:
-// the passes after it recompute whatever a changed incoming state can reach and compare bit for bit.
-#define SEC_PRED 12
+// the passes after it recompute whatever a changed incoming state can reach and compare bit for bit. The iteration
+// count is an argument (HTV_SEC=pred=...; 0 proposes pass 0's states unchanged).
+#define SEC_PRED 12                   // default iterations
 #define SEC_PRED_HALO 16
 #define SEC_PRED_T 256
 template<bool AL>
-__device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const DevTables &dt, const LineRaster *lr, const SecScratch &ss, int n, SecState (*sm)[SEC_PRED_T])
+__device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const DevTables &dt, const LineRaster *lr, const SecScratch &ss, int n, int iters,
+	SecState (*sm)[SEC_PRED_T])
 {
 	const int tid = threadIdx.x;
 	const int c = (int) blockIdx.x * (SEC_PRED_T - SEC_PRED_HALO) - SEC_PRED_HALO + tid;
@@ -327,7 +329,7 @@ __device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const 
 	sm[0][tid] = s;
 	__syncthreads();
 	#pragma unroll 1
-	for(int it = 0; it < SEC_PRED; it++)
+	for(int it = 0; it < iters; it++)
 	{
 		SecState in = (tid == 0 || c == 0) ? above : sm[it & 1][tid - 1];
 		if(clear) { in.A = 0; in.B = 0; }
@@ -344,11 +346,11 @@ __device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const 
 }
 
 __global__ void __launch_bounds__(SEC_PRED_T)
-k_sec_predict(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int n)
+k_sec_predict(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int n, int iters)
 {
 	__shared__ SecState sm[2][SEC_PRED_T];
-	if((dp.W & 7) == 0) sec_predict_body<true>(dp, dt, lr, ss, n, sm);
-	else sec_predict_body<false>(dp, dt, lr, ss, n, sm);
+	if((dp.W & 7) == 0) sec_predict_body<true>(dp, dt, lr, ss, n, iters, sm);
+	else sec_predict_body<false>(dp, dt, lr, ss, n, iters, sm);
 }
 
 // Pass >= 1: a line whose incoming state is not the one it was computed from. The IIR restarts at sample 0 and stops
@@ -439,12 +441,13 @@ k_sec_refine(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const
 // recurrence's own latency and nothing else.
 #define SEC_LIST_WARPS 4
 #define SEC_LIST_MANY 2048             // above this many lines a thread per line has the better throughput (k_sec_fm_list_t)
+// `many`: that threshold, an argument of both list kernels (HTV_SEC=list=warp / thread moves it past either end)
 __global__ void __launch_bounds__(32 * SEC_LIST_WARPS)
-k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass)
+k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass, int many)
 {
 	const int lane = threadIdx.x & 31;
 	const int nw = gridDim.x * SEC_LIST_WARPS, count = ss.flags[3];
-	if(count > SEC_LIST_MANY) return;                                       // a long list: k_sec_fm_list_t
+	if(count > many) return;                                                // a long list: k_sec_fm_list_t
 	const int W = dp.W, ck = sec_ck(W), sl = dp.burst_left;
 	const SecState *prev = ss.st[(pass + 1) & 1];
 	SecState *cur = ss.st[pass & 1];
@@ -512,11 +515,11 @@ k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, cons
 // one THREAD per listed line, 32 listed lines per warp - pass 0's arrangement, on the compacted list. FM inputs are
 // loaded two groups ahead, their look-ups issued one group ahead of the recurrence.
 __global__ void __launch_bounds__(32)
-k_sec_fm_list_t(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass)
+k_sec_fm_list_t(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass, int many)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	const int count = ss.flags[3];
-	if(count <= SEC_LIST_MANY || i >= count) return;
+	if(count <= many || i >= count) return;
 	const int c = ss.list[i];
 	const int W = dp.W, ck = sec_ck(W), G0 = ck >> 3;
 	const LineRaster &li = lr[c];

@@ -298,6 +298,22 @@ extern uint64_t htv_kernel_launches(const htv_t *s);
  * "k_sec_raster<FULL=1,MAXT=384> + k_line<...,SRC=1,...>"; "" before the first render. Read-only diagnostic:
  * the string belongs to the encoder and changes with the next render. */
 extern const char *htv_line_kernel(const htv_t *s);
+/* What the SECAM chrominance chain did since htv_init (DESIGN §6), summed over its launches; all zero for other
+ * colour modes. A launch is one sub-batch of a render call; a pass is one round of k_sec_refine + the list kernels; the
+ * work list holds the lines whose FM recurrence is re-run in full, by k_sec_fm_list (one warp per line) or, for a list
+ * longer than 2048 lines, by k_sec_fm_list_t (one thread per line). Filled from counts the chain copies to the host
+ * anyway: reading it costs no device work. */
+typedef struct {
+	int64_t launches;                     /* chain launches */
+	int64_t passes;                       /* refinement passes */
+	int64_t final_odd, final_even;        /* launches whose last pass had an odd / even number */
+	int64_t recomputed;                   /* lines k_sec_refine recomputed */
+	int64_t listed_warp, listed_thread;   /* listed lines finished by k_sec_fm_list / k_sec_fm_list_t */
+	int64_t repredict_odd, repredict_even;/* second proposals of k_sec_predict after an odd / even pass */
+	int32_t passes_max;                   /* most passes one launch needed */
+	int32_t list_max;                     /* longest work list of one pass */
+} htv_secam_chain_t;
+extern int htv_secam_chain(const htv_t *s, htv_secam_chain_t *out);
 /* Duration of the dominant kernel's (k_mod) most recent launch, measured with CUDA
  * events on the stream it ran on (0 if timing is off), and the scan lines that launch covered. */
 extern void htv_set_kernel_timing(htv_t *s, int on);
