@@ -26,6 +26,17 @@ LIB_PATH = os.environ.get("HTV_LIB") or os.path.join(_HERE, "libhacktv_b200.so")
 
 HTV_OK, HTV_ERROR, HTV_OUT_OF_MEMORY = 0, -1, -2
 
+# sample types of the rendered stream, hacktv's -t/--type (include/hacktv_b200.h HTV_TYPE_*), and their numpy dtypes
+SAMPLE_TYPES = {"uint8": 0, "int8": 1, "uint16": 2, "int16": 3, "int32": 4, "float": 5}
+SAMPLE_DTYPES = {"uint8": np.uint8, "int8": np.int8, "uint16": np.uint16, "int16": np.int16, "int32": np.int32,
+                 "float": np.float32}
+
+
+def _type_code(sample_type: str) -> int:
+    if sample_type not in SAMPLE_TYPES:
+        raise ValueError(f"unknown sample type {sample_type!r}: one of {', '.join(SAMPLE_TYPES)}")
+    return SAMPLE_TYPES[sample_type]
+
 
 class Config(C.Structure):
     """htv_config_t (include/hacktv_b200.h) = the hot-path subset of vid_config_t."""
@@ -146,6 +157,9 @@ def lib() -> C.CDLL:
     L.htv_render_host.restype = C.c_int; L.htv_render_host.argtypes = [vp, C.c_int, vp, C.POINTER(sz)]
     L.htv_render_add.restype = C.c_int; L.htv_render_add.argtypes = [vp, C.c_int, vp, C.POINTER(sz), vp]
     L.htv_mix_add.restype = C.c_int; L.htv_mix_add.argtypes = [vp, vp, sz, vp]
+    L.htv_set_sample_type.restype = C.c_int; L.htv_set_sample_type.argtypes = [vp, C.c_int]
+    L.htv_sample_type.restype = C.c_int; L.htv_sample_type.argtypes = [vp]
+    L.htv_convert.restype = C.c_int; L.htv_convert.argtypes = [vp, C.c_int, vp, sz, vp]
     L.htv_set_passthru.restype = C.c_int; L.htv_set_passthru.argtypes = [vp, _PASSTHRU_READ, vp]
     L.htv_passthru_delay_lines.restype = C.c_int; L.htv_passthru_delay_lines.argtypes = [vp]
     L.htv_set_vbi_source.restype = C.c_int; L.htv_set_vbi_source.argtypes = [vp, _READ_VBI, vp]
@@ -255,6 +269,7 @@ class Encoder:
         self.active_lines = self._L.htv_active_lines(h)
         self.complex = bool(self._L.htv_is_complex(h))
         self.bytes_per_sample = self._L.htv_bytes_per_sample(h)
+        self._sample_type = "int16"
         self.sample_rate = sample_rate
         self._keep = []
 
@@ -384,12 +399,27 @@ class Encoder:
     def passthru_delay_lines(self) -> int:
         return int(self._L.htv_passthru_delay_lines(self._h))
 
+    def set_sample_type(self, sample_type: str):
+        """htv_set_sample_type: what render / render_host write from now on ("uint8", "int8", "uint16", "int16",
+        "int32" or "float", converted as hacktv's -t/--type converts). Only before the first rendered line."""
+        if self._L.htv_set_sample_type(self._h, _type_code(sample_type)) != HTV_OK:
+            raise RuntimeError("htv_set_sample_type failed (it must precede the first rendered line)")
+        self._sample_type = sample_type
+        self.bytes_per_sample = self._L.htv_bytes_per_sample(self._h)
+
+    @property
+    def sample_type(self) -> str:
+        """The sample type render / render_host write (set_sample_type); "int16" by default."""
+        return self._sample_type
+
     def render_host(self, nlines: int, out: np.ndarray | None = None) -> np.ndarray:
-        """htv_render_host: next nlines into host memory (what `-o file` would hold)."""
+        """htv_render_host: next nlines into host memory (what `-o file -t <sample_type>` would hold), as an array of
+        the sample type's dtype."""
         per = 2 if self.complex else 1
+        dtype = SAMPLE_DTYPES[self._sample_type]
         if out is None:
-            out = np.empty(nlines * self.width * per, dtype=np.int16)
-        assert out.dtype == np.int16 and out.size >= nlines * self.width * per
+            out = np.empty(nlines * self.width * per, dtype=dtype)
+        assert out.dtype == dtype and out.size >= nlines * self.width * per
         r = self._L.htv_render_host(self._h, nlines, C.c_void_p(out.ctypes.data), None)
         if r != HTV_OK:
             raise RuntimeError(f"htv_render_host failed ({r})")
@@ -457,6 +487,14 @@ def mix_add(acc_ptr: int, in_ptr: int, nvalues: int, stream: int = 0):
     r = lib().htv_mix_add(C.c_void_p(acc_ptr), C.c_void_p(in_ptr), nvalues, C.c_void_p(stream))
     if r != HTV_OK:
         raise RuntimeError(f"htv_mix_add failed ({r})")
+
+
+def convert(dst_ptr: int, sample_type: str, src_ptr: int, nvalues: int, stream: int = 0):
+    """htv_convert: dst[i] = src[i] (int16, device memory) as `sample_type`, stream-ordered on `stream`; both
+    pointers 16-byte aligned. For a stream that already exists, e.g. a wideband sum built with render_add."""
+    r = lib().htv_convert(C.c_void_p(dst_ptr), _type_code(sample_type), C.c_void_p(src_ptr), nvalues, C.c_void_p(stream))
+    if r != HTV_OK:
+        raise RuntimeError(f"htv_convert failed ({r})")
 
 
 def test_pattern(width: int, height: int) -> np.ndarray:

@@ -1,17 +1,21 @@
 /* htv_cli - a small front end with hacktv's calling sequence (ref hacktv.c:1440-1601):
  *
- *     htv_cli -m i -s 16000000 --filter -o out.bin [--lines N] test
+ *     htv_cli -m i -s 16000000 --filter -o out.bin [-t int8] [--lines N] test
  *
  * mode lookup -> config overrides (ref hacktv.c:1107-1437, in-scope options only) ->
  * htv_init -> test source -> { htv_next_line; htv_rf_write } -> close. It exists to show
  * the C-ABI driven exactly as the reference drives video.h, and to produce files that
- * can be compared byte-for-byte with `hacktv -o file`.
+ * can be compared byte-for-byte with `hacktv -o file [-t type]`. For a sample type other
+ * than int16 the encoder converts on the device and the file is written from
+ * htv_render_host, up to one frame per call.
  */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include <signal.h>
 #include "hacktv_b200.h"
+
+static const char *const _types[] = { "uint8", "int8", "uint16", "int16", "int32", "float" };   /* HTV_TYPE_* */
 
 static volatile sig_atomic_t _abort = 0;
 static void on_signal(int sig) { (void) sig; _abort = 1; }
@@ -22,7 +26,8 @@ static void usage(void)
 		"Usage: htv_cli [options] test\n"
 		"  -m, --mode <name>      TV mode (default: i). --list-modes prints them\n"
 		"  -s, --samplerate <hz>  Sample rate (default: 16000000)\n"
-		"  -o, --output <file>    Output file, '-' for stdout (int16, IQ or real)\n"
+		"  -o, --output <file>    Output file, '-' for stdout (IQ or real)\n"
+		"  -t, --type <type>      Sample type: uint8, int8, uint16, int16 (default), int32, float\n"
 		"      --filter           Enable the VSB / low-pass video filter\n"
 		"      --nocolour --noaudio --nonicam --swap-iq\n"
 		"      --offset <hz>  --level <f>  --volume <f>\n"
@@ -33,7 +38,7 @@ int main(int argc, char **argv)
 {
 	const char *mode = "i", *out = NULL, *input = NULL;
 	unsigned int rate = 16000000, pixelrate = 0;   /* --pixelrate: raster at this rate, resampled to -s (not yet run on a GPU) */
-	int filter = 0, nocolour = 0, noaudio = 0, nonicam = 0, swap_iq = 0, i;
+	int filter = 0, nocolour = 0, noaudio = 0, nonicam = 0, swap_iq = 0, type = HTV_TYPE_INT16, i;
 	long long offset = 0, lines = -1, n = 0;
 	double level = 1.0, volume = 1.0;
 	const htv_config_t *mc;
@@ -48,6 +53,12 @@ int main(int argc, char **argv)
 		else if((!strcmp(a, "-s") || !strcmp(a, "--samplerate")) && i + 1 < argc) rate = strtoul(argv[++i], NULL, 10);
 		else if(!strcmp(a, "--pixelrate") && i + 1 < argc) pixelrate = strtoul(argv[++i], NULL, 10);
 		else if((!strcmp(a, "-o") || !strcmp(a, "--output")) && i + 1 < argc) out = argv[++i];
+		else if((!strcmp(a, "-t") || !strcmp(a, "--type")) && i + 1 < argc)
+		{
+			const char *t = argv[++i];
+			for(type = 0; type < 6 && strcmp(t, _types[type]); type++);
+			if(type == 6) { fprintf(stderr, "Unrecognised file data type.\n"); return(-1); }
+		}
 		else if(!strcmp(a, "--filter")) filter = 1;
 		else if(!strcmp(a, "--nocolour") || !strcmp(a, "--nocolor")) nocolour = 1;
 		else if(!strcmp(a, "--noaudio")) noaudio = 1;
@@ -100,6 +111,38 @@ int main(int argc, char **argv)
 		return(-1);
 	}
 	htv_info(vid);
+
+	if(type != HTV_TYPE_INT16)
+	{
+		/* the device writes the type; the file gets the bytes as they come back */
+		FILE *f;
+		char *buf;
+		const int per_frame = htv_lines_per_frame(vid);
+		size_t line_bytes;
+		int r = 0;
+		if(htv_set_sample_type(vid, type) != HTV_OK) { htv_free(vid); return(-1); }
+		line_bytes = (size_t) htv_samples_per_line(vid) * htv_bytes_per_sample(vid);   /* of the type just set */
+		if(out == NULL) { fprintf(stderr, "No output filename provided.\n"); htv_free(vid); return(-1); }
+		f = strcmp(out, "-") == 0 ? stdout : fopen(out, "wb");
+		if(!f) { perror("fopen"); htv_free(vid); return(-1); }
+		buf = malloc((size_t) per_frame * line_bytes);
+		if(buf && htv_av_test_open(htv_av(vid)) == HTV_OK)
+		{
+			while(!_abort && (lines < 0 || n < lines))
+			{
+				const int k = lines >= 0 && lines - n < per_frame ? (int) (lines - n) : per_frame;
+				if(htv_render_host(vid, k, (int16_t *) buf, NULL) != HTV_OK) { r = -1; break; }
+				if(fwrite(buf, line_bytes, (size_t) k, f) != (size_t) k) break;
+				n += k;
+			}
+		}
+		free(buf);
+		if(f != stdout) fclose(f);
+		else fflush(f);
+		htv_free(vid);
+		fprintf(stderr, "\n");
+		return(r);
+	}
 
 	if(htv_rf_file_open(&rf, out, htv_is_complex(vid)) != HTV_OK)
 	{

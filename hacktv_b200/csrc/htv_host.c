@@ -10,6 +10,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include "htv_internal.h"
+#include "htv_sample_type.h"
 
 /* Picture slots on the device and new pictures per launch sequence: with 16 slots and at most 7
  * new pictures (+ 1 carried over) per chunk, the uploads of chunk c touch no slot chunk c-1 reads,
@@ -25,6 +26,7 @@ struct htv_t {
 	htv_av_t av;
 
 	int W, lines, complex, bps;
+	int type;                     /* HTV_TYPE_* of the rendered stream (htv_set_sample_type); bps follows it */
 
 	/* stream position */
 	/* --pixelrate (ref vid_init video.c:3839, _init_vresampler 3627-3651): the raster side - tables, pictures,
@@ -157,7 +159,8 @@ int htv_init_on(htv_t **out, int device, unsigned int sample_rate, unsigned int 
 	s->W = s->tab->dp.W;
 	s->lines = s->tab->dp.lines;
 	s->complex = s->tab->dp.complex_out;
-	s->bps = s->complex ? 4 : 2;
+	s->type = HTV_TYPE_INT16;
+	s->bps = htv_st_bytes(s->type, s->complex);
 	s->cur_frame = -1;
 	s->cur_slot = -1;
 	s->av.width = s->rtab->dp.active_width;
@@ -228,6 +231,41 @@ int htv_lines_per_frame(const htv_t *s) { return(s->lines); }
 int htv_sample_rate(const htv_t *s) { return((int) s->tab->rate); }
 int htv_is_complex(const htv_t *s) { return(s->complex); }
 int htv_bytes_per_sample(const htv_t *s) { return(s->bps); }
+int htv_sample_type(const htv_t *s) { return(s ? s->type : -1); }
+
+int htv_set_sample_type(htv_t *s, int type)
+{
+	if(!s) return(HTV_ERROR);
+	if(!htv_st_size(type))
+	{
+		fprintf(stderr, "hacktv_b200: unknown sample type %d (HTV_TYPE_UINT8 .. HTV_TYPE_FLOAT)\n", type);
+		return(HTV_ERROR);
+	}
+	if(s->next_line != 0)
+	{
+		fprintf(stderr, "hacktv_b200: the sample type must be set before the first line is rendered\n");
+		return(HTV_ERROR);
+	}
+	s->type = type;
+	s->bps = htv_st_bytes(type, s->complex);
+	htv_dev_set_sample_type(s->dev, type);          /* the output context (with --pixelrate the raster side stays int16) */
+	return(HTV_OK);
+}
+
+int htv_convert(void *d_dst, int type, const int16_t *d_src, size_t nvalues, void *cuda_stream)
+{
+	if(!htv_st_size(type))
+	{
+		fprintf(stderr, "hacktv_b200: unknown sample type %d (HTV_TYPE_UINT8 .. HTV_TYPE_FLOAT)\n", type);
+		return(HTV_ERROR);
+	}
+	if(nvalues && (!d_dst || !d_src || ((uintptr_t) d_dst & 15) || ((uintptr_t) d_src & 15)))
+	{
+		fprintf(stderr, "hacktv_b200: htv_convert needs 16-byte aligned device pointers\n");
+		return(HTV_ERROR);
+	}
+	return(htv_dev_convert(d_dst, type, d_src, nvalues, cuda_stream));
+}
 int64_t htv_lines_rendered(const htv_t *s) { return(s->next_line); }
 uint64_t htv_kernel_launches(const htv_t *s) { return(htv_dev_launches(s->dev)); }
 const char *htv_line_kernel(const htv_t *s) { return(htv_dev_line_kernel(s->dev)); }
@@ -344,7 +382,8 @@ static int pull_passthru(htv_t *s, int n, void *stream)
 	lines = (int) (got / W);
 	if(lines > 0)
 	{
-		r = htv_dev_memcpy_h2d(s->dev, s->pt_dev, s->pt_host, (size_t) lines * W * s->bps, stream);
+		/* int16 in the output layout whatever the sample type: the combiner adds before the conversion */
+		r = htv_dev_memcpy_h2d(s->dev, s->pt_dev, s->pt_host, (size_t) lines * W * htv_st_bytes(HTV_TYPE_INT16, s->complex), stream);
 		if(r != HTV_OK) return(-1);
 	}
 	return(lines);
@@ -580,7 +619,7 @@ static int render_any(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, in
 		int n = nlines - done;
 		if(n > cap) n = cap;
 		if(s->pt_read && n > PT_MAX_LINES) n = PT_MAX_LINES;
-		r = render_chunk(s, &n, d_out + (size_t) done * s->W * (s->complex ? 2 : 1), add, cuda_stream);
+		r = render_chunk(s, &n, (int16_t *) ((char *) d_out + (size_t) done * s->W * s->bps), add, cuda_stream);
 		if(r != HTV_OK) return(r);
 		done += n;
 	}
@@ -595,6 +634,12 @@ int htv_render(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, void *cud
 
 int htv_render_add(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, void *cuda_stream)
 {
+	if(s && s->type != HTV_TYPE_INT16)
+	{
+		/* the sum wraps in int16; convert it once at the end (htv_convert) */
+		fprintf(stderr, "hacktv_b200: htv_render_add sums int16 streams; the sample type is %s (use htv_convert on the sum)\n", htv_st_name(s->type));
+		return(HTV_ERROR);
+	}
 	return(render_any(s, nlines, d_out, nsamples, 1, cuda_stream));
 }
 
@@ -706,6 +751,12 @@ static int frame_enqueue(htv_t *s, int buf, int n)
 htv_line_t *htv_next_line(htv_t *s)
 {
 	if(!s) return(NULL);
+	if(s->type != HTV_TYPE_INT16)
+	{
+		/* vid_next_line's contract: int16 I,Q lines (the reference's sink converts them) */
+		fprintf(stderr, "hacktv_b200: htv_next_line hands out int16 lines; the sample type is %s (use htv_render / htv_render_host)\n", htv_st_name(s->type));
+		return(NULL);
+	}
 	if(s->h_pos >= s->h_lines)
 	{
 		if(!s->h_frame[0])

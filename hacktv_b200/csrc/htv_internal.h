@@ -74,7 +74,10 @@ typedef struct {
 
 	/* FM video (ref video.c:2299-2335, 3452-3464, 3678-3740): the filtered composite + sound
 	 * carriers become the modulating signal of a Q31 phasor; pre-emphasis taps in application order */
-	int32_t have_fmv, fmv_level, fmv_ntaps, fmv_pad;
+	int32_t have_fmv, fmv_level, fmv_ntaps;
+	/* store: HTV_TYPE_* of the output stream (htv_sample_type.h), HTV_TYPE_INT16 unless htv_set_sample_type. It sits in
+	 * what was this block's padding word, so that no other field (and no kernel parameter behind dp) moves */
+	int32_t sample_type;
 	int32_t fmv_taps[HTV_FMV_MAXTAPS];
 
 	/* post mixers */
@@ -158,6 +161,8 @@ extern int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0, in
 extern void *htv_dev_event_new_timed(htv_dev_t *d);
 extern float htv_dev_event_elapsed(void *e0, void *e1);
 extern int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalues, void *stream);
+extern void htv_dev_set_sample_type(htv_dev_t *d, int type);
+extern int htv_dev_convert(void *d_dst, int type, const int16_t *d_src, size_t nvalues, void *stream);
 extern int htv_dev_memcpy_h2d(htv_dev_t *d, void *dst, const void *src, size_t bytes, void *stream);
 extern int htv_dev_sync(htv_dev_t *d, void *stream);
 extern int htv_dev_memcpy_d2h(htv_dev_t *d, void *dst, const void *src, size_t bytes, void *stream);

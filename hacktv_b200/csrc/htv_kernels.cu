@@ -24,6 +24,7 @@
 #include <stdlib.h>
 #include <limits.h>
 #include "htv_internal.h"
+#include "htv_sample_type.h"
 #include "htv_mma_fir.h"
 #include "htv_resample.h"
 
@@ -1850,6 +1851,9 @@ __device__ __forceinline__ void sound_add(const htv_dparams_t &dp, const DevTabl
 }
 
 // Mixers after the modulation (ref video.c:3466-3515), the channel combiner and the store.
+// TY: the output has another sample type than int16 (dp.sample_type, htv_sample_type.h). The kernels that share this store
+// take it as a template argument, so that their int16 instantiations compile as if the conversion did not exist.
+template<bool TY>
 __device__ __forceinline__ void post_store(const htv_dparams_t &dp, const DevTables &dt, const LineAudio &la,
 	int x0, int row, int (&oi)[SPT], int (&oq)[SPT], int16_t *out, const int16_t *acc)
 {
@@ -1897,6 +1901,20 @@ __device__ __forceinline__ void post_store(const htv_dparams_t &dp, const DevTab
 	// `acc` (same layout as `out`, may alias it): the stream to add this one into, int16 wrap per
 	// component - ref _vid_passthru_process video.c:3536-3539, the channel combiner.
 	const size_t lbase = (size_t) row * (size_t) W;
+	if constexpr(TY)
+	{
+		// another sample type: the int16 sum, then the conversion, one sample at a time; `acc` is int16 in the output
+		// layout, never `out` itself (htv_render_add refuses other types)
+		#pragma unroll
+		for(int k = 0; k < SPT; k++)
+		{
+			if(x0 + k >= W) continue;
+			const size_t s = lbase + x0 + k;
+			if(dp.complex_out) htv_st_put2(out, s, dp.sample_type, wrap16i(oi[k] + (acc ? acc[2 * s] : 0)), wrap16i(oq[k] + (acc ? acc[2 * s + 1] : 0)));
+			else htv_st_put(out, s, dp.sample_type, wrap16i(oi[k] + (acc ? acc[s] : 0)));
+		}
+		return;
+	}
 	if(dp.complex_out)
 	{
 		int16_t *o = out + (lbase + x0) * 2;
@@ -1951,7 +1969,7 @@ __device__ __forceinline__ void post_store(const htv_dparams_t &dp, const DevTab
 	}
 }
 
-template<int CSKEW>
+template<int CSKEW, bool TY>
 __device__ __forceinline__ void mod_body(const htv_dparams_t &dp, const DevTables &dt, const LineAudio &la,
 	const int *cwin, const short *ntp, int x0, int row, int16_t *out, const int16_t *acc)
 {
@@ -1990,7 +2008,7 @@ __device__ __forceinline__ void mod_body(const htv_dparams_t &dp, const DevTable
 	}
 
 	sound_add<false>(dp, dt, la, ntp, x0, oi, oq);
-	post_store(dp, dt, la, x0, row, oi, oq, out, acc);
+	post_store<TY>(dp, dt, la, x0, row, oi, oq, out, acc);
 }
 
 
@@ -2143,6 +2161,7 @@ __global__ void __launch_bounds__(1024) k_fmv_scan(const DevTables dt, int nrows
 	if(tid == 1023) *dt.fmv_carry += part[1023];
 }
 
+template<bool TY>
 __global__ void __launch_bounds__(384)
 k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, int16_t *out,
 	const int16_t *acc, int acc_rows, int out_row0)
@@ -2196,10 +2215,10 @@ k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		oi[k] = (min((int) floorf(amp * cs), 32767) * dp.fmv_level) >> 15;    // pi >> 16 <= 32767
 		oq[k] = (min((int) floorf(amp * sn), 32767) * dp.fmv_level) >> 15;
 	}
-	post_store(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
+	post_store<TY>(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
 }
 
-template<int MAXT, int MINB>
+template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, const int16_t *sadd, int16_t *out,
 	const int16_t *acc, int acc_rows)
@@ -2259,7 +2278,7 @@ k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAu
 	const int x0 = tid * SPT;
 	if(x0 >= W) return;
 
-	mod_body<0>(dp, dt, la, cw + x0 + COFF - HALO, ntp, x0, (int) blockIdx.x, out, (int) blockIdx.x < acc_rows ? acc : NULL);
+	mod_body<0, TY>(dp, dt, la, cw + x0 + COFF - HALO, ntp, x0, (int) blockIdx.x, out, (int) blockIdx.x < acc_rows ? acc : NULL);
 }
 
 // ---------------------------------------------------------------------------
@@ -2293,7 +2312,7 @@ __device__ __forceinline__ void mbar_wait(void *bar, unsigned parity)
 		:: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
-template<int MAXT, int MINB>
+template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int *comp32, int nlines, int16_t *out,
 	const int16_t *acc, int acc_rows)
@@ -2348,7 +2367,7 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		mbar_wait(&bar[cb], phase[cb]);
 		phase[cb] ^= 1;
 		const int x0 = tid * SPT;
-		if(x0 < W) mod_body<3>(dp, dt, *lab[cb], cwb[cb] + x0, ntp, x0, row, out, row < acc_rows ? acc : NULL);
+		if(x0 < W) mod_body<3, TY>(dp, dt, *lab[cb], cwb[cb] + x0, ntp, x0, row, out, row < acc_rows ? acc : NULL);
 		__syncthreads();                                            // everyone is done with this half before it is refilled
 	}
 }
@@ -2371,7 +2390,7 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 // Used whenever 128 | W, a video filter is on, and the mode is not SECAM / FM video.
 // ---------------------------------------------------------------------------
 
-template<int MAXT, int MINB>
+template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const uint8_t *planes, size_t plane_stride,
 	int pitch, int nlines, int16_t *out, const int16_t *acc, int acc_rows)
@@ -2494,7 +2513,7 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 			oi[3] = (int) (short) (v.w & 0xFFFF); oq[3] = (int) v.w >> 16;
 			const LineAudio &la = lab0[l3];
 			sound_add<false>(dp, dt, la, ntp, x0, oi, oq);
-			post_store(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
+			post_store<TY>(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
 		}
 		l3 = n3;
 	}
@@ -2709,8 +2728,8 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		return(NULL);
 	}
 	cudaFuncSetAttribute(k_raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->raster_smem);
-	cudaFuncSetAttribute(k_mod<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
-	cudaFuncSetAttribute(k_mod<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
+	cudaFuncSetAttribute(k_mod<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem); cudaFuncSetAttribute(k_mod<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
+	cudaFuncSetAttribute(k_mod<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem); cudaFuncSetAttribute(k_mod<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
 	// sub-batches keep the int16 composite scratch (2 B/sample) resident in the 50 MB L2
 	const bool secam = dp.colour_mode == HTV_SECAM;
 	// SECAM: the cross-line chain is latency bound per launch, so one launch should cover the whole call
@@ -2760,8 +2779,8 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			return(NULL);
 		}
 		cudaMemset(d->d_comp32, 0, sizeof(int) * (((size_t) d->sub_lines + 3) * W + 256));
-		cudaFuncSetAttribute(k_mod_tma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
-		cudaFuncSetAttribute(k_mod_tma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
+		cudaFuncSetAttribute(k_mod_tma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem); cudaFuncSetAttribute(k_mod_tma<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
+		cudaFuncSetAttribute(k_mod_tma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem); cudaFuncSetAttribute(k_mod_tma<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
 		d->mod_grid = nsm * (d->line_threads <= 256 ? 4 : 2);
 	}
 	if(t->rs_taps)
@@ -2803,8 +2822,8 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 				return(NULL);
 			}
 			cudaMemset(d->d_planes, 0, 2 * d->plane_stride);
-			cudaFuncSetAttribute(k_mod_mma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
-			cudaFuncSetAttribute(k_mod_mma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
+			cudaFuncSetAttribute(k_mod_mma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem); cudaFuncSetAttribute(k_mod_mma<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
+			cudaFuncSetAttribute(k_mod_mma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem); cudaFuncSetAttribute(k_mod_mma<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
 		}
 	}
 	if(secam && !dp.have_fmv && !t->raster_only && !t->rs_taps && !(getenv("HTV_PATH") && !strcmp(getenv("HTV_PATH"), "split")))
@@ -2851,7 +2870,10 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			#define KL_ATTR2(VF, HQ, FU) do { \
 				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 256, KL_B256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
 				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 320, KL_B320, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 384, KL_B384, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 384, KL_B384, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 256, KL_B256, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 320, KL_B320, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 384, KL_B384, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
 			KL_ATTR2(false, false, true); KL_ATTR2(false, false, false); KL_ATTR2(true, false, true); KL_ATTR2(true, false, false);
 			KL_ATTR2(true, true, true); KL_ATTR2(true, true, false);
 			#undef KL_ATTR2
@@ -2897,12 +2919,16 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			#define KL_ATTR2(VF, HQ, FU, CS) do { \
 				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 256, KL_B256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
 				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 320, KL_B320>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 384, KL_B384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 384, KL_B384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 256, KL_B256, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 320, KL_B320, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
+				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 384, KL_B384, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
 			#define KL_ATTR(VF, HQ) do { KL_ATTR2(VF, HQ, true, false); KL_ATTR2(VF, HQ, false, false); KL_ATTR2(VF, HQ, false, true); } while(0)
 			KL_ATTR(false, false); KL_ATTR(true, false); KL_ATTR(true, true);
 			#undef KL_ATTR
 			#undef KL_ATTR2
 			cudaFuncSetAttribute(k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem);
+			cudaFuncSetAttribute(k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem);
 		}
 	}
 	if(secam)
@@ -3199,10 +3225,15 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 }
 
 // The instantiation of the fused line kernel a launch uses, every template argument spelled out (htv_line_kernel); written
-// next to each launch, so that a change to the selection shows up in the name
-static void kl_name(char *s, size_t n, bool vf, bool hq, bool full, bool csat, int maxt, bool src, int snd, int wc)
+// next to each launch, so that a change to the selection shows up in the name. The int16 forms keep their names; a store
+// that converts appends its sample type: ",ST=int8" compiled in, ",ST=-1:float" converting to dp.sample_type at run time.
+static void kl_name(char *s, size_t n, bool vf, bool hq, bool full, bool csat, int maxt, bool src, int snd, int wc,
+	int st = HTV_TYPE_INT16, int dyn_type = HTV_TYPE_INT16)
 {
-	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d>", vf, hq, full, csat, maxt, src, snd, wc);
+	char ts[24] = "";
+	if(st < 0) snprintf(ts, sizeof(ts), ",ST=-1:%s", htv_st_name(dyn_type));
+	else if(st != HTV_TYPE_INT16) snprintf(ts, sizeof(ts), ",ST=%s", htv_st_name(st));
+	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d%s>", vf, hq, full, csat, maxt, src, snd, wc, ts);
 }
 
 extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int16_t *d_out,
@@ -3273,9 +3304,12 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		if(run < 4) run = 4;
 		const int grid = (nlines + run - 1) / run;
 		if(d->timing) cudaEventRecord(d->ev0, st);
+		// another sample type than int16: the same forms with the store converting to dp.sample_type
+		const bool typed = dp.sample_type != HTV_TYPE_INT16;
 		#define KL_GO3(VF, HQ, FU, CS, T, B) do { \
-			kl_name(d->kname, sizeof(d->kname), VF, HQ, FU, CS, T, false, -1, 0); \
-			k_line<VF, HQ, FU, CS, T, B><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); } while(0)
+			kl_name(d->kname, sizeof(d->kname), VF, HQ, FU, CS, T, false, -1, 0, typed ? -1 : HTV_TYPE_INT16, dp.sample_type); \
+			if(typed) k_line<VF, HQ, FU, CS, T, B, false, -1, 0, -1><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); \
+			else k_line<VF, HQ, FU, CS, T, B><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); } while(0)
 		#define KL_GO2(VF, HQ, FU, CS) do { \
 			if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, CS, 256, KL_B256); \
 			else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, CS, 320, KL_B320); \
@@ -3285,11 +3319,13 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			else if(!d->kl_csat) KL_GO2(VF, HQ, false, false); else KL_GO2(VF, HQ, false, true); } while(0)
 		if(!dp.vf_type) KL_GO(false, false);
 		// ... and within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those sound stages
-		// and the width compiled in
-		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !d->kl_general)
+		// and the width compiled in, storing int16 or int8 (the HackRF's format); other sample types run the general form
+		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !d->kl_general &&
+			(dp.sample_type == HTV_TYPE_INT16 || dp.sample_type == HTV_TYPE_INT8))
 		{
-			kl_name(d->kname, sizeof(d->kname), true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024);
-			k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
+			kl_name(d->kname, sizeof(d->kname), true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, dp.sample_type);
+			if(typed) k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
+			else k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
 		}
 		else if(dp.vf_type == 3) KL_GO(true, true);
 		else KL_GO(true, false);
@@ -3327,11 +3363,12 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 	d->launches += 2;
 	d->side_armed = 0;
 	bool joined = false;
+	const bool typed = d->dp.sample_type != HTV_TYPE_INT16;         // the modulators' store converts (post_store<true>)
 	for(int done = 0; done < nlines; done += d->sub_lines)
 	{
 		const int n = nlines - done < d->sub_lines ? nlines - done : d->sub_lines;
 		const bool last = done + n >= nlines;
-		int16_t *o = d_out + (size_t) done * d->dp.W * (d->dp.complex_out ? 2 : 1);
+		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * d->dp.W * htv_st_bytes(d->dp.sample_type, d->dp.complex_out));
 		const int16_t *sadd = NULL;
 		const int16_t *cstream = d->d_comp;
 		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
@@ -3462,7 +3499,8 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			else if(dp.fmv_ntaps == 0) k_fmv_base<0><<<rows, d->line_threads, d->fmv_smem, st>>>(dp, d->dt, lap, cstream, sadd, pre);
 			else { fprintf(stderr, "hacktv_b200: unsupported FM pre-emphasis length %d\n", dp.fmv_ntaps); return(HTV_ERROR); }
 			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, rows);
-			k_fmv_mod<<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
+			if(typed) k_fmv_mod<true><<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
+			else k_fmv_mod<false><<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
 			snprintf(mname, sizeof(mname), "k_fmv_base<%d> + k_fmv_scan + k_fmv_mod", dp.fmv_ntaps);
 			d->launches += 2;
 		}
@@ -3474,8 +3512,9 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			if(run < 4) run = 4;
 			const int grid = (n + run - 1) / run;
 			#define KL_GO3(VF, HQ, FU, T, B) do { \
-				kl_name(mname, sizeof(mname), VF, HQ, FU, false, T, true, -1, 0); \
-				k_line<VF, HQ, FU, false, T, B, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); } while(0)
+				kl_name(mname, sizeof(mname), VF, HQ, FU, false, T, true, -1, 0, typed ? -1 : HTV_TYPE_INT16, dp.sample_type); \
+				if(typed) k_line<VF, HQ, FU, false, T, B, true, -1, 0, -1><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); \
+				else k_line<VF, HQ, FU, false, T, B, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); } while(0)
 			#define KL_GO2(VF, HQ, FU) do { \
 				if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, 256, KL_B256); \
 				else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, 320, KL_B320); \
@@ -3491,18 +3530,20 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		else if(d->d_planes)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_mma<256,4>"); k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); }
-			else { snprintf(mname, sizeof(mname), "k_mod_mma<384,2>"); k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); }
+			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_mma<256,4>"); { if(typed) k_mod_mma<256, 4, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); else k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); } }
+			else { snprintf(mname, sizeof(mname), "k_mod_mma<384,2>"); { if(typed) k_mod_mma<384, 2, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); } }
 		}
 		else if(d->d_comp32)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_tma<256,4>"); k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); }
-			else { snprintf(mname, sizeof(mname), "k_mod_tma<384,2>"); k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); }
+			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_tma<256,4>"); { if(typed) k_mod_tma<256, 4, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); } }
+			else { snprintf(mname, sizeof(mname), "k_mod_tma<384,2>"); { if(typed) k_mod_tma<384, 2, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); } }
 		}
-		else if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod<256,4>"); k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); }
-		else { snprintf(mname, sizeof(mname), "k_mod<384,2>"); k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); }
-		snprintf(d->kname, sizeof(d->kname), "%s + %s", rname, mname);
+		else if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod<256,4>"); { if(typed) k_mod<256, 4, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); else k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); } }
+		else { snprintf(mname, sizeof(mname), "k_mod<384,2>"); { if(typed) k_mod<384, 2, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); } }
+		// a modulator whose store converts: its template argument TY, with the type (k_line spells its own)
+		snprintf(d->kname, sizeof(d->kname), "%s + %s%s%s", rname, mname, typed && !d->sec_line ? " ST=-1:" : "",
+			typed && !d->sec_line ? htv_st_name(d->dp.sample_type) : "");
 		d->launches++;
 		if(last) d->last_mod_lines = n;
 	}
@@ -3596,6 +3637,7 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	CK(cudaEventRecord(d->ev_audio, d->side));
 	d->side_armed = 0;
 	bool joined = false;
+	const bool typed = d->dp.sample_type != HTV_TYPE_INT16;         // the modulators' store converts (post_store<true>)
 	d->launches += 2;
 	const int Ws = d->dp.W, Wp = r->dp.W;
 	int sub = d->sub_lines < r->sub_lines ? d->sub_lines : r->sub_lines;
@@ -3603,7 +3645,7 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	{
 		const int n = nlines - done < sub ? nlines - done : sub;
 		const bool last = done + n >= nlines;
-		int16_t *o = d_out + (size_t) done * Ws * (d->dp.complex_out ? 2 : 1);
+		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * Ws * htv_st_bytes(d->dp.sample_type, d->dp.complex_out));
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * Ws * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
 		// raster lines line0 + done - 1 .. line0 + done + n + 1 -> rows 0 .. n + 2 of the raster context's int16 stream
@@ -3617,20 +3659,20 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 		if(d->d_planes)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows);
-			else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows);
+			if(d->line_threads <= 256) { if(typed) k_mod_mma<256, 4, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); else k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); }
+			else { if(typed) k_mod_mma<384, 2, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); }
 		}
 		else if(d->d_comp32)
 		{
 			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows);
-			else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows);
+			if(d->line_threads <= 256) { if(typed) k_mod_tma<256, 4, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); }
+			else { if(typed) k_mod_tma<384, 2, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); }
 		}
-		else if(d->line_threads <= 256) k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows);
-		else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows);
+		else if(d->line_threads <= 256) { if(typed) k_mod<256, 4, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); else k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); }
+		else { if(typed) k_mod<384, 2, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); }
 		d->launches++;
-		snprintf(d->kname, sizeof(d->kname), "k_raster + k_resample + %s<%d,%d>", d->d_planes ? "k_mod_mma" : d->d_comp32 ? "k_mod_tma" : "k_mod",
-			d->line_threads <= 256 ? 256 : 384, d->line_threads <= 256 ? 4 : 2);
+		snprintf(d->kname, sizeof(d->kname), "k_raster + k_resample + %s<%d,%d>%s%s", d->d_planes ? "k_mod_mma" : d->d_comp32 ? "k_mod_tma" : "k_mod",
+			d->line_threads <= 256 ? 256 : 384, d->line_threads <= 256 ? 4 : 2, typed ? " ST=-1:" : "", typed ? htv_st_name(d->dp.sample_type) : "");
 		if(last) d->last_mod_lines = n;
 	}
 	if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
@@ -3679,6 +3721,77 @@ extern "C" int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalu
 	if(blocks > (size_t) nsm * 8) blocks = (size_t) nsm * 8;
 	if(blocks < 1) blocks = 1;
 	k_mix_add<<<(unsigned) blocks, 256, 0, (cudaStream_t) stream>>>(d_acc, d_in, nvalues);
+	CK(cudaGetLastError());
+	return(HTV_OK);
+}
+
+// The sample type the stores convert to (htv_set_sample_type): read from dp at every launch
+extern "C" void htv_dev_set_sample_type(htv_dev_t *d, int type) { d->dp.sample_type = type; }
+
+// htv_convert: dst[i] = the `type` form of src[i] (htv_sample_type.h), eight values per thread and step: one 16-byte
+// load, one store of 8, 16 or 32 bytes
+template<int T>
+__global__ void __launch_bounds__(256) k_convert(void *dst, const int16_t *src, size_t nvalues)
+{
+	constexpr int S = T == HTV_TYPE_INT8 || T == HTV_TYPE_UINT8 ? 1 : (T == HTV_TYPE_INT32 || T == HTV_TYPE_FLOAT ? 4 : 2);
+	const size_t n8 = nvalues / 8;
+	const size_t stride = (size_t) gridDim.x * blockDim.x;
+	for(size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += stride)
+	{
+		const int4 a = __ldcs(reinterpret_cast<const int4 *>(src) + i);
+		const int v[8] = { (short) a.x, a.x >> 16, (short) a.y, a.y >> 16, (short) a.z, a.z >> 16, (short) a.w, a.w >> 16 };
+		if(S == 1)
+		{
+			uint2 o;
+			o.x = htv_st_bits(T, v[0]) | (htv_st_bits(T, v[1]) << 8) | (htv_st_bits(T, v[2]) << 16) | (htv_st_bits(T, v[3]) << 24);
+			o.y = htv_st_bits(T, v[4]) | (htv_st_bits(T, v[5]) << 8) | (htv_st_bits(T, v[6]) << 16) | (htv_st_bits(T, v[7]) << 24);
+			__stcs(reinterpret_cast<uint2 *>(dst) + i, o);
+		}
+		else if(S == 2)
+		{
+			const uint4 o = make_uint4(htv_st_bits(T, v[0]) | (htv_st_bits(T, v[1]) << 16), htv_st_bits(T, v[2]) | (htv_st_bits(T, v[3]) << 16),
+				htv_st_bits(T, v[4]) | (htv_st_bits(T, v[5]) << 16), htv_st_bits(T, v[6]) | (htv_st_bits(T, v[7]) << 16));
+			__stcs(reinterpret_cast<uint4 *>(dst) + i, o);
+		}
+		else
+		{
+			__stcs(reinterpret_cast<uint4 *>(dst) + 2 * i, make_uint4(htv_st_bits(T, v[0]), htv_st_bits(T, v[1]), htv_st_bits(T, v[2]), htv_st_bits(T, v[3])));
+			__stcs(reinterpret_cast<uint4 *>(dst) + 2 * i + 1, make_uint4(htv_st_bits(T, v[4]), htv_st_bits(T, v[5]), htv_st_bits(T, v[6]), htv_st_bits(T, v[7])));
+		}
+	}
+	if(blockIdx.x == 0 && threadIdx.x < (nvalues & 7))
+	{
+		const size_t i = n8 * 8 + threadIdx.x;
+		htv_st_put(dst, i, T, src[i]);
+	}
+}
+
+extern "C" int htv_dev_convert(void *d_dst, int type, const int16_t *d_src, size_t nvalues, void *stream)
+{
+	if(!htv_st_size(type) || (((uintptr_t) d_dst) | ((uintptr_t) d_src)) & 15) return(HTV_ERROR);
+	if(!nvalues) return(HTV_OK);
+	int dev = 0, nsm = 132;
+	cudaGetDevice(&dev);
+	{
+		// run where the destination lives
+		cudaPointerAttributes pa;
+		if(cudaPointerGetAttributes(&pa, d_dst) == cudaSuccess && pa.type == cudaMemoryTypeDevice) dev = pa.device;
+	}
+	DevGuard guard(dev);
+	cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+	size_t blocks = (nvalues / 8 + 255) / 256;
+	if(blocks > (size_t) nsm * 8) blocks = (size_t) nsm * 8;
+	if(blocks < 1) blocks = 1;
+	cudaStream_t st = (cudaStream_t) stream;
+	switch(type)
+	{
+	case HTV_TYPE_UINT8: k_convert<HTV_TYPE_UINT8><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	case HTV_TYPE_INT8: k_convert<HTV_TYPE_INT8><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	case HTV_TYPE_UINT16: k_convert<HTV_TYPE_UINT16><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	case HTV_TYPE_INT16: k_convert<HTV_TYPE_INT16><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	case HTV_TYPE_INT32: k_convert<HTV_TYPE_INT32><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	case HTV_TYPE_FLOAT: k_convert<HTV_TYPE_FLOAT><<<(unsigned) blocks, 256, 0, st>>>(d_dst, d_src, nvalues); break;
+	}
 	CK(cudaGetLastError());
 	return(HTV_OK);
 }

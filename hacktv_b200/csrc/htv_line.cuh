@@ -201,8 +201,12 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 	}
 }
 
-// Mixers after the modulation (ref video.c:3466-3515), channel combiner, store - post_store for the strided layout
-template<bool FULL, int SND>
+// Mixers after the modulation (ref video.c:3466-3515), channel combiner, store - post_store for the strided layout.
+// ST: the sample type the store converts to (htv_sample_type.h), -1 for dp.sample_type at run time. The channel combiner
+// (`acc`, int16 in the output layout) still adds in int16 with wrap-around; the conversion is the last step, as the
+// reference's file sink converts what the video stage handed it. A lane stores each of its samples on its own (1, 2,
+// 4 or 8 bytes); the eight lanes g = 0..7 of a t still cover one contiguous run of the line per j.
+template<bool FULL, int SND, int ST>
 __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
 	int W, int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
 {
@@ -241,6 +245,22 @@ __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const Dev
 		}
 	}
 	const size_t lbase = (size_t) row * (size_t) W;
+	if constexpr(ST != HTV_TYPE_INT16)
+	{
+		const int st = ST < 0 ? dp.sample_type : ST;
+		const bool cpx = KL_HAS(SND, KL_CPX, dp.complex_out);
+		#pragma unroll
+		for(int j = 0; j < 4; j++)
+		{
+			if(FULL || xb + 8 * j < W)
+			{
+				const size_t s = lbase + xb + 8 * j;
+				if(cpx) htv_st_put2(out, s, st, wrap16i(oi[j] + (acc ? acc[2 * s] : 0)), wrap16i(oq[j] + (acc ? acc[2 * s + 1] : 0)));
+				else htv_st_put(out, s, st, wrap16i(oi[j] + (acc ? acc[s] : 0)));
+			}
+		}
+		return;
+	}
 	if(KL_HAS(SND, KL_CPX, dp.complex_out))
 	{
 		unsigned *o = reinterpret_cast<unsigned *>(out) + lbase + xb;
@@ -288,7 +308,8 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 // SRC: the composite lines are not rastered here but read from `src` (row q + 2 = relative line q, int16): SECAM, whose
 // chrominance chain (htv_secam.cuh) runs between the raster and the modulator. R1b / R2 fold away, the rest is the same.
 // WC: the line width compiled in (0: dp.W), so that the shared-memory row and plane offsets become immediates
-template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0>
+// ST: the output sample type compiled into the store (HTV_TYPE_INT16: the int16 store), -1: dp.sample_type at run time
+template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap,
 	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr)
@@ -564,7 +585,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		{
 			const LineA2 *la = sla + (mrow & 1);
 			kl_sound<SND>(dp, dt, la, ntp, xb, oi, oq);
-			kl_post_store<FULL, SND>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
+			kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
 		}
 	}
 	#undef KL_R1A

@@ -378,6 +378,7 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 	dp->raster = c->type;
 	dp->colour_mode = c->colour_mode;
 	dp->complex_out = c->output_type == HTV_INT16_COMPLEX;
+	dp->sample_type = HTV_TYPE_INT16;
 	dp->interlaced = c->interlaced;
 	dp->volume = c->volume;
 	dp->swap_iq = c->swap_iq;

@@ -46,6 +46,13 @@ extern "C" {
 /* output_type (ref rf.h:26-28) */
 #define HTV_INT16_COMPLEX 0
 #define HTV_INT16_REAL    1
+/* sample type of the rendered stream, as the file sink's -t/--type (ref rf.h:31-36); htv_set_sample_type */
+#define HTV_TYPE_UINT8  0
+#define HTV_TYPE_INT8   1
+#define HTV_TYPE_UINT16 2
+#define HTV_TYPE_INT16  3
+#define HTV_TYPE_INT32  4
+#define HTV_TYPE_FLOAT  5
 /* modulation (ref video.h:71-74) */
 #define HTV_NONE 0
 #define HTV_AM   1
@@ -255,9 +262,24 @@ extern int htv_set_prefetch(htv_t *s, int on);
  * of samples produced. `d_out` must be 16-byte aligned (the kernels store, and htv_render_add
  * also loads, 128 bits at a time); a misaligned pointer is refused with HTV_ERROR. Output layout is what the reference's file sink writes
  * (rf_file.c:97-116, 226-233): int16 I,Q interleaved for complex modes, int16
- * I only for real modes. */
+ * I only for real modes. With htv_set_sample_type the buffer holds that type
+ * instead (the pointer keeps its int16_t type; size it in bytes). */
 extern int htv_render(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, void *cuda_stream);
 extern int htv_render_host(htv_t *s, int nlines, int16_t *h_out, size_t *nsamples);
+
+/* Sample type of what htv_render / htv_render_host write: HTV_TYPE_UINT8 .. HTV_TYPE_FLOAT, each value converted
+ * from the int16 the encoder computes exactly as the reference's file sink converts it (ref rf_file.c, -t/--type):
+ * uint8 (x + 32768) >> 8, int8 x >> 8, uint16 x + 32768, int32 x * 65537, float x / 32767 (rounded from a double
+ * product). The conversion is the last step of the store, after --offset and the channel combiner (htv_set_passthru
+ * still adds in int16). Default HTV_TYPE_INT16. Allowed only before the first line is rendered; an unknown type is
+ * refused. htv_bytes_per_sample follows it. htv_render_add (an int16 sum) and htv_next_line (int16 lines, as
+ * vid_next_line) refuse any other type. */
+extern int htv_set_sample_type(htv_t *s, int type);
+extern int htv_sample_type(const htv_t *s);
+/* d_dst[i] = the `type` form of d_src[i] over nvalues int16 values in device memory (I and Q alike), stream-ordered
+ * on cuda_stream. Both pointers 16-byte aligned. For streams that already exist: a wideband sum built with
+ * htv_render_add, converted once at the end. */
+extern int htv_convert(void *d_dst, int type, const int16_t *d_src, size_t nvalues, void *cuda_stream);
 
 /* Channel combiner - replaces the reference's `--passthru` stage (vid_config_t.passthru
  * video.h:158; _vid_passthru_process video.c:3517-3541, set-up 4607-4634): an external int16
@@ -289,13 +311,15 @@ extern int htv_active_lines(const htv_t *s);
 extern int htv_lines_per_frame(const htv_t *s);
 extern int htv_sample_rate(const htv_t *s);
 extern int htv_is_complex(const htv_t *s);
-extern int htv_bytes_per_sample(const htv_t *s);   /* 4 complex, 2 real */
+extern int htv_bytes_per_sample(const htv_t *s);   /* int16: 4 complex, 2 real; other sample types their size */
 extern int64_t htv_lines_rendered(const htv_t *s);
 /* Kernel launches issued by this encoder since htv_init (for bench accounting) */
 extern uint64_t htv_kernel_launches(const htv_t *s);
 /* The line kernel(s) the most recent render launched, with their template arguments, e.g.
  * "k_line<VF=1,HQ=1,FULL=0,CSAT=1,MAXT=384,SRC=0,SND=-1,WC=0>", or for SECAM
- * "k_sec_raster<FULL=1,MAXT=384> + k_line<...,SRC=1,...>"; "" before the first render. Read-only diagnostic:
+ * "k_sec_raster<FULL=1,MAXT=384> + k_line<...,SRC=1,...>"; "" before the first render. A store that converts to
+ * another sample type than int16 appends it: ",ST=int8" compiled in, ",ST=-1:float" chosen at run time (k_line), or
+ * " ST=-1:float" after the split, FM-video and --pixelrate modulators. Read-only diagnostic:
  * the string belongs to the encoder and changes with the next render. */
 extern const char *htv_line_kernel(const htv_t *s);
 /* What the SECAM chrominance chain did since htv_init (DESIGN §6), summed over its launches; all zero for other
