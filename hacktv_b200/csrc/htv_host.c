@@ -246,9 +246,10 @@ int htv_set_sample_type(htv_t *s, int type)
 		fprintf(stderr, "hacktv_b200: the sample type must be set before the first line is rendered\n");
 		return(HTV_ERROR);
 	}
+	/* the output context (with --pixelrate the raster side stays int16) */
+	if(htv_dev_set_sample_type(s->dev, type) != HTV_OK) return(HTV_ERROR);
 	s->type = type;
 	s->bps = htv_st_bytes(type, s->complex);
-	htv_dev_set_sample_type(s->dev, type);          /* the output context (with --pixelrate the raster side stays int16) */
 	return(HTV_OK);
 }
 

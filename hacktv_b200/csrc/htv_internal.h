@@ -161,7 +161,11 @@ extern int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0, in
 extern void *htv_dev_event_new_timed(htv_dev_t *d);
 extern float htv_dev_event_elapsed(void *e0, void *e1);
 extern int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalues, void *stream);
-extern void htv_dev_set_sample_type(htv_dev_t *d, int type);
+/* the kernels of the new type's stores (before the first rendered line); HTV_ERROR with a message on stderr */
+extern int htv_dev_set_sample_type(htv_dev_t *d, int type);
+/* the name htv_line_kernel would report for an encoder of these tables writing this sample type, under the switches
+ * (HTV_PATH, HTV_FIR, HTV_KL) in the environment; the kernel selection alone, without a CUDA call (CPU tests) */
+extern int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, char *name, size_t len);
 extern int htv_dev_convert(void *d_dst, int type, const int16_t *d_src, size_t nvalues, void *stream);
 extern int htv_dev_memcpy_h2d(htv_dev_t *d, void *dst, const void *src, size_t bytes, void *stream);
 extern int htv_dev_sync(htv_dev_t *d, void *stream);

@@ -22,13 +22,13 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdlib.h>
+#include <stdarg.h>
 #include <limits.h>
 #include "htv_internal.h"
 #include "htv_sample_type.h"
 #include "htv_mma_fir.h"
 #include "htv_resample.h"
 
-#define HTV_FIR_DEFAULT_MMA 1         // the tensor-core video filter is the default where it applies (HTV_FIR=scalar turns it off)
 #define HALO 25                       // (HTV_VF_NTAPS - 1) / 2
 #define RA_BITS 20
 #define RA (1 << RA_BITS)             // audio ring: pairs / processed samples / phase prefix
@@ -144,14 +144,45 @@ struct SecScratch {
 #define HTV_MAX_ALLOCS 128            // device tables owned by one encoder (about 50 for SECAM-L with AM + NICAM)
 #define HTV_OV_CAP 2048                // VBI overlay lines per launch sequence
 
+// The A/B and test switches, read from the environment once per encoder (dev_switches), beside HTV_SEC (sec_knobs)
+struct DevSwitches {
+	bool split;                       // HTV_PATH=split: the separate raster + modulator kernels where the fused ones would run
+	bool scalar;                      // HTV_FIR=scalar: the scalar video filter and SECAM notch, not the tensor-core ones
+	bool kl_general;                  // HTV_KL=general: never the k_line with the sound stages and width compiled in
+	bool no_ahead;                    // HTV_AHEAD=0: the fused line kernel's sound pre-pass in the caller's stream order
+	bool debug;                       // HTV_DEBUG: the SECAM chain's passes on stderr
+};
+
+// What an encoder launches (plan_kernels): chosen once from its tables, the switches and the sample type
+enum { PATH_LINE, PATH_SEC_LINE, PATH_SPLIT, PATH_FMV, PATH_RS, PATH_RASTER };
+struct KLine; struct KSec; struct KMod; struct KFmvBase; struct KFmvMod;
+struct DevPlan {
+	int path;                         // LINE: k_line; SEC_LINE: SECAM raster + chain + k_line<SRC>; SPLIT: raster (+ chain) +
+	                                  // modulator; FMV: raster (+ chain) + FM video; RS / RASTER: the two sides of --pixelrate
+	const KLine *kl;                  // LINE, SEC_LINE
+	const KSec *ks;                   // SEC_LINE: the SECAM raster on the tensor cores; NULL: k_raster_secam
+	const KMod *mod;                  // SPLIT, RS
+	const KFmvBase *fmv_base;         // FMV
+	const KFmvMod *fmv_mod;
+	const void *raster;               // k_raster or k_raster_secam where this context launches one
+	size_t raster_smem, kl_smem, ks_smem, mod_smem, fmv_smem;   // their dynamic shared memory
+	int line_threads;                 // CTA of the split kernels: a thread per 4 samples, whole warps, at least 64
+	int kl_threads;                   // CTA of the fused kernels: a warp per tile of 128 samples
+	int plane_pitch;                  // k_mod_mma: 0, the planes are the contiguous stream; else bytes per line row (htv_mma_fir.h)
+	char kname[192];                  // what htv_line_kernel reports once a render has launched the plan
+};
+
 struct htv_dev_t {
 	int device;
+	const struct htv_tables_t *tab;   // the encoder's tables (they outlive it): plan_kernels again on a new sample type
+	DevSwitches sw;
+	DevPlan plan;
 	htv_dparams_t dp;
 	DevTables dt;
 	size_t frame_pixels;
 	int max_slots;
 	void *alloc[HTV_MAX_ALLOCS];
-	int nalloc;
+	int nalloc, alloc_failed;
 	uint32_t *d_frames;
 	int32_t *d_frame_map;
 	int frame_map_cap;
@@ -186,35 +217,25 @@ struct htv_dev_t {
 	int r2_armed;
 	int side_armed;
 	int ev_pending;
-	int line_threads;
 	void *d_desc_r, *d_desc_a;        // LineRaster[cap + 2], LineAudio[cap]
 	void *d_desc_r2, *d_desc_a2;      // LineR2[cap + 2], LineA2[cap] (fused line kernel)
 	void *d_desc_s2;                  // LineS2[cap + 3] (SECAM raster in the fused kernel's form)
 	int desc_cap;
-	// the fused line kernel (htv_line.cuh): PAL / NTSC / mono, AM or VSB, no resampler
-	int use_line, kl_threads, kl_ctas, kl_csat;
-	int kl_general;                   // HTV_KL=general: never the instantiation with the sound stages and width compiled in
+	int kl_ctas;                      // persistent CTAs of the fused kernels (k_line, k_sec_raster)
 	char kname[192];                  // the line kernel(s) the last render launched, with their template arguments (htv_line_kernel)
-	int sec_line;                     // SECAM: the modulator is the fused line kernel in its SRC form (composite rows from d_comp)
-	size_t ks_smem;                   // ... and the raster is k_sec_raster (0: k_raster_secam)
-	size_t kl_smem;
 	SecScratch sec;                   // SECAM scratch (same sub-batch rows as d_comp)
 	// the SECAM chain's switches (HTV_SEC, sec_knobs) and what it did since the encoder was created (htv_secam_chain)
 	int sec_passes, sec_pred, sec_many, sec_repredict, sec_repredict_min, sec_sub;
 	htv_secam_chain_t sec_stats;
 	int *d_comp32;                    // int32 composite scratch for the TMA-fed modulator (4 | W, not SECAM)
-	uint8_t *d_planes;                // high / low byte planes of the composite stream for k_mod_mma (32 | W, video filter on)
-	size_t plane_stride, modm_smem;
-	int plane_pitch;                  // 0: planes are the contiguous stream; else bytes per line row (htv_mma_fir.h)
+	uint8_t *d_planes;                // high / low byte planes of the composite stream for k_mod_mma (video filter on)
+	size_t plane_stride;
 	// --pixelrate: this is the sample-rate side; the raster runs in a second context at the pixel rate
 	int rs_I, rs_D, rs_ataps, rs_wp;
 	int16_t *d_rs_taps;
-	size_t modt_smem;
-	int mod_grid;
+	int mod_grid;                     // persistent CTAs of k_mod_tma / k_mod_mma
 	int16_t *d_comp;                  // composite scratch, (sub + 3) lines, reused by every sub-batch (stays in L2)
 	int sub_lines;
-	size_t fmv_smem;
-	size_t raster_smem, mod_smem;
 	int last_mod_lines;
 };
 
@@ -2050,7 +2071,7 @@ __device__ __forceinline__ unsigned long long block_sum_u64(unsigned long long v
 
 template<int NT>
 __global__ void __launch_bounds__(384)
-k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, const int16_t *sadd, int pre)
+k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, int pre)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = dp.W;
@@ -2078,18 +2099,11 @@ k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const L
 		// b * W when row 0 is the pipeline's fill line (`pre`), whose history is zero
 		const size_t r = (size_t) blockIdx.x + 1 - pre;
 		const int16_t *cs = comp + r * W;
-		const int16_t *sa = sadd ? sadd + r * W : NULL;
 		const bool first = pre && blockIdx.x == 0;
 		for(int i = tid; i < CW; i += blockDim.x)
 		{
 			const int x = i - FOFF;
-			int v = 0;
-			if(!(first && x < 0))
-			{
-				v = __ldg(cs + x);
-				if(sa) v = wrap16i(v + __ldg(sa + x));              // SECAM subcarrier of the same stream position
-			}
-			cw[i] = v;
+			cw[i] = first && x < 0 ? 0 : __ldg(cs + x);
 		}
 	}
 	__syncthreads();
@@ -2220,7 +2234,7 @@ k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 
 template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
-k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, const int16_t *sadd, int16_t *out,
+k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, int16_t *out,
 	const int16_t *acc, int acc_rows)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -2261,13 +2275,6 @@ k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAu
 			{
 				#pragma unroll
 				for(int k = 0; k < 4; k++) v[k] = __ldg(cs + xe0 + k);
-			}
-			if(sadd)
-			{
-				// SECAM: the subcarrier samples k_secam_seq produced for the same stream positions
-				const int16_t *sa = sadd + ((size_t) blockIdx.x + 1) * W + xe0;
-				#pragma unroll
-				for(int k = 0; k < 4; k++) v[k] = wrap16i(v[k] + __ldg(sa + k));
 			}
 			#pragma unroll
 			for(int k = 0; k < 4; k++) cw[xe0 + k + COFF] = v[k];
@@ -2536,15 +2543,90 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 #include "htv_secam_raster.cuh"
 
 // ---------------------------------------------------------------------------
+// Kernel tables: every instantiation the host launches, with its entry point taken by address and its template arguments
+// as data. Each table's macro passes the same literals to the template and to the entry, so that the selection
+// (plan_kernels), the launch and the name htv_line_kernel reports all come from one entry.
+// ---------------------------------------------------------------------------
+
+// resident CTAs per SM of a persistent line kernel of MAXT threads
+#define KL_MINB(T) ((T) <= 256 ? KL_B256 : (T) <= 320 ? KL_B320 : KL_B384)
+
+typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, int, int, int16_t *, const int16_t *, int, const int16_t *);
+struct KLine { KLineFn fn; int vf, hq, full, csat, maxt, minb, src, snd, wc, st; };
+#define KL_ENTRY(VF, HQ, FU, CS, T, SRC, SND, WC, ST) \
+	{ k_line<VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST>, VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST }
+// at each CTA size, the int16 store and the store converting to dp.sample_type at run time
+#define KL_MAXT(VF, HQ, FU, CS, SRC) \
+	KL_ENTRY(VF, HQ, FU, CS, 256, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 256, SRC, -1, 0, -1), \
+	KL_ENTRY(VF, HQ, FU, CS, 320, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 320, SRC, -1, 0, -1), \
+	KL_ENTRY(VF, HQ, FU, CS, 384, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 384, SRC, -1, 0, -1)
+// no video filter, a real low-pass, VSB
+#define KL_VF(FU, CS, SRC) KL_MAXT(false, false, FU, CS, SRC), KL_MAXT(true, false, FU, CS, SRC), KL_MAXT(true, true, FU, CS, SRC)
+static const KLine kl_tab[] = {
+	KL_VF(true, false, false), KL_VF(false, false, false), KL_VF(false, true, false),   // 128 | W, a partial last tile, CSAT
+	KL_VF(true, false, true), KL_VF(false, false, true),                                // SECAM's SRC form: 128 | W, partial
+	// PAL's VSB + FM + NICAM + complex output and W = 1024 (16 Msps) compiled in, storing int16 or int8 (the HackRF's format)
+	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT16),
+	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8),
+};
+
+typedef void (*KSecFn)(htv_dparams_t, DevTables, const LineS2 *, int, int, int16_t *, SecScratch);
+struct KSec { KSecFn fn; int full, maxt, minb; };
+#define KS_ENTRY(FU, T) { k_sec_raster<FU, T, KL_MINB(T)>, FU, T, KL_MINB(T) }
+static const KSec ks_tab[] = {
+	KS_ENTRY(true, 256), KS_ENTRY(false, 256), KS_ENTRY(true, 320), KS_ENTRY(false, 320), KS_ENTRY(true, 384), KS_ENTRY(false, 384),
+};
+
+// the split modulators: k_mod (int16 stream), k_mod_tma (int32 stream, 4 | W), k_mod_mma (byte planes, video filter on);
+// an entry has the entry point of its own kernel only
+typedef void (*KModFn)(htv_dparams_t, DevTables, const LineAudio *, const int16_t *, int16_t *, const int16_t *, int);
+typedef void (*KModTmaFn)(htv_dparams_t, DevTables, const LineAudio *, const int *, int, int16_t *, const int16_t *, int);
+typedef void (*KModMmaFn)(htv_dparams_t, DevTables, const LineAudio *, const uint8_t *, size_t, int, int, int16_t *, const int16_t *, int);
+struct KMod { const char *name; KModFn mod; KModTmaFn tma; KModMmaFn mma; int maxt, minb, ty; };
+#define KM_ENTRY(T, B, TY) \
+	{ "k_mod", k_mod<T, B, TY>, NULL, NULL, T, B, TY }, { "k_mod_tma", NULL, k_mod_tma<T, B, TY>, NULL, T, B, TY }, \
+	{ "k_mod_mma", NULL, NULL, k_mod_mma<T, B, TY>, T, B, TY }
+static const KMod km_tab[] = { KM_ENTRY(256, 4, false), KM_ENTRY(256, 4, true), KM_ENTRY(384, 2, false), KM_ENTRY(384, 2, true) };
+
+typedef void (*KFmvBaseFn)(htv_dparams_t, DevTables, const LineAudio *, const int16_t *, int);
+struct KFmvBase { KFmvBaseFn fn; int nt; };
+#define KFB_ENTRY(NT) { k_fmv_base<NT>, NT }
+static const KFmvBase kfb_tab[] = { KFB_ENTRY(0), KFB_ENTRY(67), KFB_ENTRY(71) };
+
+typedef void (*KFmvModFn)(htv_dparams_t, DevTables, const LineAudio *, int16_t *, const int16_t *, int, int);
+struct KFmvMod { KFmvModFn fn; int ty; };
+#define KFM_ENTRY(TY) { k_fmv_mod<TY>, TY }
+static const KFmvMod kfm_tab[] = { KFM_ENTRY(false), KFM_ENTRY(true) };
+
+// the entry of tab that match accepts; none counts a miss
+template<typename E, size_t N, typename F> static const E *kfind(const E (&tab)[N], int &miss, F match)
+{
+	for(const E &e : tab) if(match(e)) return(&e);
+	miss++;
+	return(NULL);
+}
+
+// The name of a k_line instantiation, every template argument spelled out (htv_line_kernel). The int16 forms keep their
+// names; a store that converts appends its sample type: ",ST=int8" compiled in, ",ST=-1:float" converting at run time.
+static void kl_name(char *s, size_t n, const KLine &k, int type)
+{
+	char ts[24] = "";
+	if(k.st < 0) snprintf(ts, sizeof(ts), ",ST=-1:%s", htv_st_name(type));
+	else if(k.st != HTV_TYPE_INT16) snprintf(ts, sizeof(ts), ",ST=%s", htv_st_name(k.st));
+	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d%s>", k.vf, k.hq, k.full, k.csat, k.maxt, k.src, k.snd, k.wc, ts);
+}
+
+// ---------------------------------------------------------------------------
 // Device layer (C linkage)
 // ---------------------------------------------------------------------------
 
+// A failed allocation sets alloc_failed, which fails htv_dev_create; a missing table (src NULL) is not a failure
 static void *dev_copy(htv_dev_t *d, const void *src, size_t bytes)
 {
 	void *p = NULL;
-	if(!src || !bytes || d->nalloc >= HTV_MAX_ALLOCS) return(NULL);
-	if(cudaMalloc(&p, bytes) != cudaSuccess) return(NULL);
-	if(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(p); return(NULL); }
+	if(!src || !bytes) return(NULL);
+	if(d->nalloc >= HTV_MAX_ALLOCS || cudaMalloc(&p, bytes) != cudaSuccess) { d->alloc_failed = 1; return(NULL); }
+	if(cudaMemcpy(p, src, bytes, cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(p); d->alloc_failed = 1; return(NULL); }
 	d->alloc[d->nalloc++] = p;
 	return(p);
 }
@@ -2552,8 +2634,8 @@ static void *dev_copy(htv_dev_t *d, const void *src, size_t bytes)
 static void *dev_zero(htv_dev_t *d, size_t bytes)
 {
 	void *p = NULL;
-	if(d->nalloc >= HTV_MAX_ALLOCS || cudaMalloc(&p, bytes) != cudaSuccess) return(NULL);
-	if(cudaMemset(p, 0, bytes) != cudaSuccess) { cudaFree(p); return(NULL); }
+	if(d->nalloc >= HTV_MAX_ALLOCS || cudaMalloc(&p, bytes) != cudaSuccess) { d->alloc_failed = 1; return(NULL); }
+	if(cudaMemset(p, 0, bytes) != cudaSuccess) { cudaFree(p); d->alloc_failed = 1; return(NULL); }
 	d->alloc[d->nalloc++] = p;
 	return(p);
 }
@@ -2616,6 +2698,178 @@ static bool sec_knobs(htv_dev_t *d, char *err, size_t errlen)
 	return(true);
 }
 
+static DevSwitches dev_switches(void)
+{
+	const char *path = getenv("HTV_PATH"), *fir = getenv("HTV_FIR"), *kl = getenv("HTV_KL"), *ahead = getenv("HTV_AHEAD");
+	DevSwitches s;
+	s.split = path && !strcmp(path, "split");
+	s.scalar = fir && !strcmp(fir, "scalar");
+	s.kl_general = kl && !strcmp(kl, "general");
+	s.no_ahead = ahead && !strcmp(ahead, "0");
+	s.debug = getenv("HTV_DEBUG") != NULL;
+	return(s);
+}
+
+// The kernels an encoder launches, from its tables, the switches and the output sample type alone - never from what the
+// device could allocate: the path, the table entries it launches, their shared memory and the name htv_line_kernel
+// reports. Host code without a CUDA call (htv_dev_plan_name runs it on a machine without a GPU).
+static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int type, DevPlan *p, char *err, size_t errlen)
+{
+	const htv_dparams_t &dp = t->dp;
+	const int W = dp.W, W4 = (W + 3) & ~3, T = mf_tiles(W);
+	const bool secam = dp.colour_mode == HTV_SECAM, typed = type != HTV_TYPE_INT16, full = W % MF_TILE == 0;
+	const size_t ntp = sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7);     // the padded NICAM pulse table in shared memory
+	memset(p, 0, sizeof(*p));
+	p->line_threads = ((W + 3) / 4 + 31) & ~31;
+	if(p->line_threads < 64) p->line_threads = 64;
+	p->kl_threads = 32 * T;
+	if(p->line_threads > 384) { snprintf(err, errlen, "line width %d exceeds the kernels' 1536-sample limit", W); return(HTV_ERROR); }
+	if(secam && t->rs_taps) { snprintf(err, errlen, "--pixelrate with SECAM is not on the accelerated path yet"); return(HTV_ERROR); }
+	// The fused line kernel (htv_line.cuh) is the default wherever it applies: PAL / NTSC / mono rasters, AM or VSB
+	// modulation (or baseband), a chroma low-pass the tensor-core form holds (11 .. 17 taps), no resampler in front of
+	// this context. SECAM: its SRC form modulates what the raster and the chrominance chain wrote.
+	const bool chroma_ok = dp.colour_mode == HTV_MONOCHROME ||
+		((dp.colour_mode == HTV_PAL || dp.colour_mode == HTV_NTSC) && dp.chroma_ntaps >= 3 && dp.chroma_ntaps <= 17);
+	// the video filter on the tensor cores (k_mod_mma, k_line), the default for every line width: multiples of 128
+	// through the contiguous byte planes, the rest (NTSC 858, 864, ...) through the pitched plane layout (htv_mma_fir.h)
+	const bool mma = !secam && dp.vf_type && !sw.scalar;
+	if(t->raster_only) p->path = PATH_RASTER;
+	else if(dp.have_fmv) p->path = PATH_FMV;
+	else if(t->rs_taps) p->path = PATH_RS;
+	else if(secam && !sw.split) p->path = PATH_SEC_LINE;
+	else if(!secam && !sw.split && chroma_ok && (!dp.vf_type || mma) && t->tmpl_out) p->path = PATH_LINE;
+	else p->path = PATH_SPLIT;
+
+	p->raster_smem = sizeof(int) * 2 * (W4 + 2 * UOFF);
+	if(secam)
+	{
+		const size_t sm = sizeof(int) * ((((W4 + 2 * LOFF + 14) + 3) & ~3) + W4 + 32) + 2 * (size_t) mf_row_bytes(W) + 32;
+		if(sm > p->raster_smem) p->raster_smem = sm;
+	}
+	const void *raster = secam ? (const void *) k_raster_secam : (const void *) k_raster;
+	const int maxt = p->kl_threads <= 256 ? 256 : p->kl_threads <= 320 ? 320 : 384;
+	const int vf = dp.vf_type != 0, hq = dp.vf_type == 3, kst = typed ? -1 : HTV_TYPE_INT16;
+	const size_t rowb = (size_t) mf_row_bytes(W) + 16, uvb = (size_t) MF_TILE * T + 32;
+	int miss = 0;                                    // instantiations the rule asks for and the tables lack
+	switch(p->path)
+	{
+	case PATH_LINE:
+	{
+		// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768. The Gaussian taps are
+		// rounded one by one, so at about 1 % of sample rates they sum to 32769 .. 32771 (17.734475, 20.05 Msps: 32769),
+		// and those rates run the CSAT form
+		long long sum = 0;
+		for(int i = 0; i < dp.chroma_ntaps; i++) sum += dp.chroma_taps[i] < 0 ? -dp.chroma_taps[i] : dp.chroma_taps[i];
+		const int csat = sum > 32768;
+		// the common case (128 | W, a chroma filter that cannot overflow) has its own instantiation, everything else the
+		// general one; within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those
+		// sound stages and the width compiled in, storing int16 or int8; other sample types run the general form
+		const bool fixed = hq && !csat && W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !sw.kl_general &&
+			(type == HTV_TYPE_INT16 || type == HTV_TYPE_INT8);
+		p->kl = kfind(kl_tab, miss, [&](const KLine &k) {
+			return(k.vf == vf && k.hq == hq && k.full == (full && !csat) && k.csat == csat && k.maxt == maxt && !k.src &&
+				k.snd == (fixed ? KL_SND_FM_NICAM : -1) && k.wc == (fixed ? W : 0) && k.st == (fixed ? type : kst)); });
+		break;
+	}
+	case PATH_SEC_LINE:
+		p->kl = kfind(kl_tab, miss, [&](const KLine &k) {
+			return(k.vf == vf && k.hq == hq && k.full == full && !k.csat && k.maxt == maxt && k.src && k.snd == -1 && !k.wc && k.st == kst); });
+		// the raster with the luma notch on the tensor cores (k_sec_raster); HTV_FIR=scalar: k_raster_secam
+		if(!sw.scalar && t->tmpl_out)
+		{
+			p->ks = kfind(ks_tab, miss, [&](const KSec &k) { return(k.full == full && k.maxt == maxt); });
+			p->ks_smem = 2 * sizeof(LineS2) + 4 * rowb + 4 * uvb + sizeof(uint4) * (MF_KSTEPS * 2 * 32 + 64) + 64;
+		}
+		else p->raster = raster;
+		break;
+	case PATH_SPLIT:
+	case PATH_RS:
+	{
+		// k_mod_mma where the video filter runs on the tensor cores, else k_mod_tma where 4 | W, else k_mod
+		const bool tma = !mma && !secam && (W & 3) == 0;
+		const char *name = mma ? "k_mod_mma" : tma ? "k_mod_tma" : "k_mod";
+		const int mt = p->line_threads <= 256 ? 256 : 384;
+		p->mod = kfind(km_tab, miss, [&](const KMod &k) { return(!strcmp(k.name, name) && k.maxt == mt && k.ty == typed); });
+		if(mma)
+		{
+			p->plane_pitch = full ? 0 : mf_pitch(W);
+			p->mod_smem = (size_t) 4 * (p->plane_pitch ? mf_row_bytes(W) : mf_plane_bytes(W)) + sizeof(uint32_t) * MF_ATAB_WORDS +
+				sizeof(unsigned) * 2 * mf_tiles(W) * 4 * MF_ROWW + 3 * sizeof(LineAudio) + ntp + 128;
+		}
+		else if(tma) p->mod_smem = sizeof(int) * 2 * TWIN(W) + 2 * sizeof(LineAudio) + ntp + 128;
+		else p->mod_smem = sizeof(int) * (W4 + 2 * EXT + 16) + ntp;
+		// --pixelrate: the raster runs in the pixel-rate context (PATH_RASTER), k_resample brings it to this one
+		if(p->path == PATH_SPLIT) p->raster = raster;
+		break;
+	}
+	case PATH_FMV:
+		p->raster = raster;
+		p->fmv_base = kfind(kfb_tab, miss, [&](const KFmvBase &k) { return(k.nt == dp.fmv_ntaps); });
+		p->fmv_mod = kfind(kfm_tab, miss, [&](const KFmvMod &k) { return(k.ty == typed); });
+		p->fmv_smem = sizeof(int) * (W4 + 2 * FOFF) + ntp;
+		if(!p->fmv_base) { snprintf(err, errlen, "unsupported FM pre-emphasis length %d", dp.fmv_ntaps); return(HTV_ERROR); }
+		break;
+	case PATH_RASTER:
+		p->raster = (const void *) k_raster;
+		break;
+	}
+	if(miss) { snprintf(err, errlen, "no kernel instantiation for path %d at W = %d", p->path, W); return(HTV_ERROR); }
+
+	// the name: a split modulator whose store converts appends its TY with the type (k_line spells its own)
+	const char *rname = p->ks ? "k_sec_raster" : p->path == PATH_RS ? "k_raster + k_resample" : secam ? "k_raster_secam" : "k_raster";
+	char kl[128] = "", tail[24] = "";
+	snprintf(tail, sizeof(tail), typed ? " ST=-1:%s" : "", htv_st_name(type));
+	if(p->kl)
+	{
+		kl_name(kl, sizeof(kl), *p->kl, type);
+		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 + ntp + 128;
+	}
+	if(p->path == PATH_LINE) snprintf(p->kname, sizeof(p->kname), "%s", kl);
+	else if(p->ks) snprintf(p->kname, sizeof(p->kname), "%s<FULL=%d,MAXT=%d> + %s", rname, p->ks->full, p->ks->maxt, kl);
+	else if(p->kl) snprintf(p->kname, sizeof(p->kname), "%s + %s", rname, kl);
+	else if(p->mod) snprintf(p->kname, sizeof(p->kname), "%s + %s<%d,%d>%s", rname, p->mod->name, p->mod->maxt, p->mod->minb, tail);
+	else if(p->fmv_base) snprintf(p->kname, sizeof(p->kname), "%s + k_fmv_base<%d> + k_fmv_scan + k_fmv_mod%s", rname, p->fmv_base->nt, tail);
+	return(HTV_OK);
+}
+
+// Gives each kernel of the plan the dynamic shared memory it launches with
+static bool plan_attributes(const DevPlan &p, char *err, size_t errlen)
+{
+	const KMod *m = p.mod;
+	const struct { const void *fn; size_t smem; } k[] = {
+		{ p.raster, p.raster_smem },
+		{ p.kl ? (const void *) p.kl->fn : NULL, p.kl_smem },
+		{ p.ks ? (const void *) p.ks->fn : NULL, p.ks_smem },
+		{ !m ? NULL : m->mma ? (const void *) m->mma : m->tma ? (const void *) m->tma : (const void *) m->mod, p.mod_smem },
+		{ p.fmv_base ? (const void *) p.fmv_base->fn : NULL, p.fmv_smem },
+	};
+	for(const auto &e : k)
+	{
+		const cudaError_t r = e.fn ? cudaFuncSetAttribute(e.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) e.smem) : cudaSuccess;
+		if(r != cudaSuccess) { snprintf(err, errlen, "%s: %zu bytes of shared memory refused (%s)", p.kname, e.smem, cudaGetErrorString(r)); return(false); }
+	}
+	return(true);
+}
+
+extern "C" int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, char *name, size_t len)
+{
+	DevPlan p;
+	if(plan_kernels(t, dev_switches(), sample_type, &p, name, len) != HTV_OK) return(HTV_ERROR);
+	snprintf(name, len, "%s", p.kname);
+	return(HTV_OK);
+}
+
+// htv_dev_create's way out: the message, and everything allocated so far freed
+static htv_dev_t *create_fail(htv_dev_t *d, char *err, size_t errlen, const char *fmt, ...)
+{
+	va_list ap;
+	va_start(ap, fmt);
+	vsnprintf(err, errlen, fmt, ap);
+	va_end(ap);
+	htv_dev_destroy(d);
+	return(NULL);
+}
+
 extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame_slots, int device, char *err, size_t errlen)
 {
 	int n = 0;
@@ -2635,9 +2889,12 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	htv_dev_t *d = (htv_dev_t *) calloc(1, sizeof(htv_dev_t));
 	if(!d) { snprintf(err, errlen, "out of memory"); return(NULL); }
 	d->device = device;
+	d->tab = t;
 	d->dp = t->dp;
-	if(!sec_knobs(d, err, errlen)) { free(d); return(NULL); }
+	d->sw = dev_switches();
+	if(!sec_knobs(d, err, errlen) || plan_kernels(t, d->sw, d->dp.sample_type, &d->plan, err, errlen) != HTV_OK) { free(d); return(NULL); }
 	const htv_dparams_t &dp = d->dp;
+	const DevPlan &p = d->plan;
 	DevTables &dt = d->dt;
 
 	dt.codes = (const uint16_t *) dev_copy(d, t->codes, sizeof(uint16_t) * t->ncodes);
@@ -2666,11 +2923,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	{
 		short4 *lut = NULL;
 		if(!dt.glut || cudaMalloc((void **) &lut, sizeof(short4) << 24) != cudaSuccess)
-		{
-			snprintf(err, errlen, "device allocation failed (RGB -> YUV table, 134 MB)");
-			htv_dev_destroy(d);
-			return(NULL);
-		}
+			return(create_fail(d, err, errlen, "device allocation failed (RGB -> YUV table, 134 MB)"));
 		d->alloc[d->nalloc++] = lut;
 		if(dp.colour_mode == HTV_SECAM) k_yuv_lut<true><<<65536, 256>>>(dp, dt.glut, lut);
 		else k_yuv_lut<false><<<65536, 256>>>(dp, dt.glut, lut);
@@ -2704,34 +2957,15 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		dt.nic_ftot = (uint8_t *) dev_zero(d, RF);
 		dt.nic_fstart = (uint8_t *) dev_zero(d, RF);
 	}
-	if(!d->d_frames || !d->d_pcm || !dt.codes || !d->h_map || cudaGetLastError() != cudaSuccess)
-	{
-		snprintf(err, errlen, "device allocation failed");
-		htv_dev_destroy(d);
-		return(NULL);
-	}
+	if(!dt.codes || !d->h_map || d->alloc_failed || cudaGetLastError() != cudaSuccess) return(create_fail(d, err, errlen, "device allocation failed"));
 	d->fm_jc = -1;
 	d->nic_kc = 0;
 
 	const int W = dp.W;
-	int threads = (W + 3) / 4;
-	threads = (threads + 31) & ~31;
-	if(threads < 64) threads = 64;
-	d->line_threads = threads;
-	const int W4 = (W + 3) & ~3;
-	d->raster_smem = sizeof(int) * 2 * (W4 + 2 * UOFF);
-	d->mod_smem = sizeof(int) * (W4 + 2 * EXT + 16) + sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7);
-	if(threads > 384)
-	{
-		snprintf(err, errlen, "line width %d exceeds the kernels' 1536-sample limit", W);
-		htv_dev_destroy(d);
-		return(NULL);
-	}
-	cudaFuncSetAttribute(k_raster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->raster_smem);
-	cudaFuncSetAttribute(k_mod<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem); cudaFuncSetAttribute(k_mod<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
-	cudaFuncSetAttribute(k_mod<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem); cudaFuncSetAttribute(k_mod<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->mod_smem);
-	// sub-batches keep the int16 composite scratch (2 B/sample) resident in the 50 MB L2
 	const bool secam = dp.colour_mode == HTV_SECAM;
+	int nsm = 132;
+	cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
+	// sub-batches keep the int16 composite scratch (2 B/sample) resident in the 50 MB L2
 	// SECAM: the cross-line chain is latency bound per launch, so one launch should cover the whole call
 	d->sub_lines = ((secam ? 160 : 16) * 1024 * 1024) / (W * 2);
 	if(d->sub_lines < 64) d->sub_lines = 64;
@@ -2739,201 +2973,63 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	{
 		// HTV_SEC=sub=...: shorter chain launches, so that a call crosses launch boundaries (tests)
 		if(d->sec_sub > d->sub_lines)
-		{
-			snprintf(err, errlen, "HTV_SEC: sub=%d is more than the %d lines of one launch", d->sec_sub, d->sub_lines);
-			htv_dev_destroy(d);
-			return(NULL);
-		}
+			return(create_fail(d, err, errlen, "HTV_SEC: sub=%d is more than the %d lines of one launch", d->sec_sub, d->sub_lines));
 		d->sub_lines = d->sec_sub;
 	}
-	if(cudaMalloc((void **) &d->d_comp, sizeof(int16_t) * ((size_t) d->sub_lines + 3) * W + 256) != cudaSuccess)
+	const size_t rows = (size_t) d->sub_lines + 3;
+	if(p.path != PATH_LINE && cudaMalloc((void **) &d->d_comp, sizeof(int16_t) * rows * W + 256) != cudaSuccess)
+		return(create_fail(d, err, errlen, "device allocation failed"));
+	if(p.path == PATH_FMV)
 	{
-		snprintf(err, errlen, "device allocation failed");
-		htv_dev_destroy(d);
-		return(NULL);
-	}
-	if(dp.have_fmv)
-	{
-		const size_t rows = (size_t) d->sub_lines + 4;
-		dt.fmv_base = (int16_t *) dev_zero(d, sizeof(int16_t) * rows * W + 256);
-		dt.fmv_tot = (unsigned long long *) dev_zero(d, sizeof(unsigned long long) * rows);
-		dt.fmv_rowbase = (unsigned long long *) dev_zero(d, sizeof(unsigned long long) * rows);
+		dt.fmv_base = (int16_t *) dev_zero(d, sizeof(int16_t) * (rows + 1) * W + 256);
+		dt.fmv_tot = (unsigned long long *) dev_zero(d, sizeof(unsigned long long) * (rows + 1));
+		dt.fmv_rowbase = (unsigned long long *) dev_zero(d, sizeof(unsigned long long) * (rows + 1));
 		dt.fmv_carry = (unsigned long long *) dev_zero(d, sizeof(unsigned long long));
-		d->fmv_smem = sizeof(int) * (W4 + 2 * FOFF) + sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7);
-		if(!dt.fmv_ang || !dt.fmv_base || !dt.fmv_tot || !dt.fmv_rowbase || !dt.fmv_carry)
-		{
-			snprintf(err, errlen, "device allocation failed");
-			htv_dev_destroy(d);
-			return(NULL);
-		}
+		if(!dt.fmv_ang) return(create_fail(d, err, errlen, "FM video without its modulator table"));
 	}
-	if(!secam && (W & 3) == 0 && !dp.have_fmv && !t->raster_only)
+	if(p.mod && p.mod->tma)
 	{
-		int nsm = 132;
-		cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
-		d->modt_smem = sizeof(int) * 2 * TWIN(W) + 2 * sizeof(LineAudio) + sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
-		if(cudaMalloc((void **) &d->d_comp32, sizeof(int) * (((size_t) d->sub_lines + 3) * W + 256)) != cudaSuccess)
-		{
-			snprintf(err, errlen, "device allocation failed");
-			htv_dev_destroy(d);
-			return(NULL);
-		}
-		cudaMemset(d->d_comp32, 0, sizeof(int) * (((size_t) d->sub_lines + 3) * W + 256));
-		cudaFuncSetAttribute(k_mod_tma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem); cudaFuncSetAttribute(k_mod_tma<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
-		cudaFuncSetAttribute(k_mod_tma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem); cudaFuncSetAttribute(k_mod_tma<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modt_smem);
-		d->mod_grid = nsm * (d->line_threads <= 256 ? 4 : 2);
+		const size_t bytes = sizeof(int) * (rows * W + 256);
+		if(cudaMalloc((void **) &d->d_comp32, bytes) != cudaSuccess) return(create_fail(d, err, errlen, "device allocation failed"));
+		cudaMemset(d->d_comp32, 0, bytes);
 	}
-	if(t->rs_taps)
+	if(p.mod && p.mod->mma)
+	{
+		d->plane_stride = rows * (p.plane_pitch ? p.plane_pitch : W) + 256;
+		if(cudaMalloc((void **) &d->d_planes, 2 * d->plane_stride) != cudaSuccess) return(create_fail(d, err, errlen, "device allocation failed"));
+		cudaMemset(d->d_planes, 0, 2 * d->plane_stride);
+	}
+	if(p.mod) d->mod_grid = nsm * p.mod->minb;
+	if(p.kl) d->kl_ctas = nsm * p.kl->minb;
+	if(p.path == PATH_RS)
 	{
 		d->rs_I = t->rs_I; d->rs_D = t->rs_D; d->rs_ataps = t->rs_ataps; d->rs_wp = t->rs_wp;
 		d->d_rs_taps = (int16_t *) dev_copy(d, t->rs_taps, sizeof(int16_t) * t->rs_I * t->rs_ataps);
-		if(!d->d_rs_taps || secam)
-		{
-			snprintf(err, errlen, secam ? "--pixelrate with SECAM is not on the accelerated path yet" : "device allocation failed");
-			htv_dev_destroy(d);
-			return(NULL);
-		}
 	}
-	if(!secam && !dp.have_fmv && dp.vf_type && !t->raster_only)
+	// the tap operands of the tensor-core filters the plan's kernels read
+	if((p.kl && p.kl->vf) || (p.mod && p.mod->mma))
 	{
-		// the video filter on the tensor cores (k_mod_mma), the default for every line width: multiples of
-		// 128 through the contiguous byte planes, the rest (NTSC 858, 864, ...) through the pitched plane
-		// layout (htv_mma_fir.h) - both validated against the scalar filter and the oracle
-		// (tests/test_gpu_zz_mma_fir.py). HTV_FIR=scalar selects the scalar kernels (A/B runs, tests)
-		const char *sel = getenv("HTV_FIR");
-		const bool want_mma = sel ? strcmp(sel, "scalar") != 0 : HTV_FIR_DEFAULT_MMA;
-		if(want_mma)
-		{
-			int nsm = 132;
-			cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
-			d->mod_grid = nsm * (d->line_threads <= 256 ? 4 : 2);
-			uint32_t atab[MF_ATAB_WORDS];
-			mf_build_atab(dp.vf_i, dp.vf_q, atab);
-			d->dt.mma_atab = (const uint32_t *) dev_copy(d, atab, sizeof(atab));
-			d->plane_pitch = W % MF_TILE == 0 ? 0 : mf_pitch(W);
-			d->plane_stride = ((size_t) d->sub_lines + 3) * (d->plane_pitch ? d->plane_pitch : W) + 256;
-			d->modm_smem = (size_t) 4 * (d->plane_pitch ? mf_row_bytes(W) : mf_plane_bytes(W)) + sizeof(uint32_t) * MF_ATAB_WORDS +
-				sizeof(unsigned) * 2 * mf_tiles(W) * 4 * MF_ROWW + 3 * sizeof(LineAudio) +
-				sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
-			if(!d->dt.mma_atab || cudaMalloc((void **) &d->d_planes, 2 * d->plane_stride) != cudaSuccess)
-			{
-				snprintf(err, errlen, "device allocation failed");
-				htv_dev_destroy(d);
-				return(NULL);
-			}
-			cudaMemset(d->d_planes, 0, 2 * d->plane_stride);
-			cudaFuncSetAttribute(k_mod_mma<256, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem); cudaFuncSetAttribute(k_mod_mma<256, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
-			cudaFuncSetAttribute(k_mod_mma<384, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem); cudaFuncSetAttribute(k_mod_mma<384, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->modm_smem);
-		}
+		uint32_t atab[MF_ATAB_WORDS];
+		mf_build_atab(dp.vf_i, dp.vf_q, atab);
+		dt.mma_atab = (const uint32_t *) dev_copy(d, atab, sizeof(atab));
 	}
-	if(secam && !dp.have_fmv && !t->raster_only && !t->rs_taps && !(getenv("HTV_PATH") && !strcmp(getenv("HTV_PATH"), "split")))
+	if(secam && !d->sw.scalar)
 	{
-		// SECAM: raster and chrominance chain write the composite rows, the fused line kernel's SRC form modulates them
-		int nsm = 132;
-		cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
-		if(dp.vf_type)
-		{
-			uint32_t atab[MF_ATAB_WORDS];
-			mf_build_atab(dp.vf_i, dp.vf_q, atab);
-			d->dt.mma_atab = (const uint32_t *) dev_copy(d, atab, sizeof(atab));
-		}
-		if(!dp.vf_type || d->dt.mma_atab)
-		{
-			const int T = mf_tiles(W);
-			d->kl_threads = 32 * T;
-			d->kl_ctas = nsm * (d->kl_threads <= 256 ? KL_B256 : (d->kl_threads <= 320 ? KL_B320 : KL_B384));
-			const size_t rowb = (size_t) mf_row_bytes(W) + 16, uvb = (size_t) MF_TILE * T + 32;
-			d->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (dp.vf_type ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 +
-				sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
-			d->sec_line = 1;
-			if(!(getenv("HTV_FIR") && !strcmp(getenv("HTV_FIR"), "scalar")))
-			{
-				uint32_t nt[MF_KSTEPS * 2 * 32 * 4];
-				for(int s3 = 0; s3 < MF_KSTEPS; s3++) for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
-					nt[((s3 * 2 + lo) * 32 + lane) * 4 + reg] = mf_a_word(dp.secam_notch, s3, lane, reg, lo);
-				d->dt.notch_atab = (const uint32_t *) dev_copy(d, nt, sizeof(nt));
-			}
-			if(d->dt.notch_atab && dt.tmpl_out)
-			{
-				uint32_t ctab[256];
-				for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
-					ctab[(lo * 32 + lane) * 4 + reg] = kl_chroma_a_word(dp.secam_lpf, 15, lane, reg, lo);
-				d->dt.sec_lpf_atab = (const uint32_t *) dev_copy(d, ctab, sizeof(ctab));
-				d->ks_smem = 2 * sizeof(LineS2) + 4 * rowb + 4 * uvb + sizeof(uint4) * (MF_KSTEPS * 2 * 32 + 64) + 64;
-				cudaFuncSetAttribute(k_sec_raster<true, 256, KL_B256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-				cudaFuncSetAttribute(k_sec_raster<false, 256, KL_B256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-				cudaFuncSetAttribute(k_sec_raster<true, 320, KL_B320>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-				cudaFuncSetAttribute(k_sec_raster<false, 320, KL_B320>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-				cudaFuncSetAttribute(k_sec_raster<true, 384, KL_B384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-				cudaFuncSetAttribute(k_sec_raster<false, 384, KL_B384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->ks_smem);
-			}
-			#define KL_ATTR2(VF, HQ, FU) do { \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 256, KL_B256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 320, KL_B320, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 384, KL_B384, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 256, KL_B256, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 320, KL_B320, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, false, 384, KL_B384, true, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
-			KL_ATTR2(false, false, true); KL_ATTR2(false, false, false); KL_ATTR2(true, false, true); KL_ATTR2(true, false, false);
-			KL_ATTR2(true, true, true); KL_ATTR2(true, true, false);
-			#undef KL_ATTR2
-		}
+		uint32_t nt[MF_KSTEPS * 2 * 32 * 4];
+		for(int s3 = 0; s3 < MF_KSTEPS; s3++) for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
+			nt[((s3 * 2 + lo) * 32 + lane) * 4 + reg] = mf_a_word(dp.secam_notch, s3, lane, reg, lo);
+		dt.notch_atab = (const uint32_t *) dev_copy(d, nt, sizeof(nt));
 	}
-	{
-		// The fused line kernel (htv_line.cuh) is the default wherever it applies: PAL / NTSC / mono rasters, AM or
-		// VSB modulation (or baseband), a chroma low-pass the tensor-core form holds (11 .. 17 taps), no resampler
-		// in front of this context. HTV_PATH=split selects the separate raster + modulator kernels (A/B runs, tests).
-		const char *sel = getenv("HTV_PATH");
-		const bool split = sel && !strcmp(sel, "split");
-		const bool chroma_ok = dp.colour_mode == HTV_MONOCHROME ||
-			((dp.colour_mode == HTV_PAL || dp.colour_mode == HTV_NTSC) && dp.chroma_ntaps >= 3 && dp.chroma_ntaps <= 17);
-		const bool vf_ok = dp.vf_type == 0 || d->dt.mma_atab != NULL;
-		if(!split && !secam && !dp.have_fmv && !t->raster_only && !t->rs_taps && chroma_ok && vf_ok && dt.tmpl_out)
-		{
-			int nsm = 132;
-			cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, d->device);
-			const int T = mf_tiles(W);
-			d->kl_threads = 32 * T;
-			d->kl_ctas = nsm * (d->kl_threads <= 256 ? KL_B256 : (d->kl_threads <= 320 ? KL_B320 : KL_B384));
-			if(dp.colour_mode != HTV_MONOCHROME)
-			{
-				uint32_t ctab[256];
-				for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
-					ctab[(lo * 32 + lane) * 4 + reg] = kl_chroma_a_word(dp.chroma_taps, dp.chroma_ntaps, lane, reg, lo);
-				d->dt.chroma_atab = (const uint32_t *) dev_copy(d, ctab, sizeof(ctab));
-			}
-			const size_t rowb = (size_t) mf_row_bytes(W) + 16, uvb = (size_t) MF_TILE * T + 32;
-			d->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (dp.vf_type ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 +
-				sizeof(short) * ((dp.nicam_tpad_len + 7) & ~7) + 128;
-			d->use_line = 1;
-			// HTV_KL=general: the general instantiation where the one with the sound stages compiled in would run (A/B, tests)
-			d->kl_general = getenv("HTV_KL") && !strcmp(getenv("HTV_KL"), "general");
-			{
-				// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768. The Gaussian taps are
-				// rounded one by one, so at about 1 % of sample rates they sum to 32769 .. 32771 (17.734475, 20.05 Msps: 32769),
-				// and those rates run the CSAT form
-				long long sum = 0;
-				for(int i = 0; i < dp.chroma_ntaps; i++) sum += dp.chroma_taps[i] < 0 ? -dp.chroma_taps[i] : dp.chroma_taps[i];
-				d->kl_csat = sum > 32768;
-			}
-			#define KL_ATTR2(VF, HQ, FU, CS) do { \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 256, KL_B256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 320, KL_B320>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 384, KL_B384>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 256, KL_B256, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 320, KL_B320, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); \
-				cudaFuncSetAttribute(k_line<VF, HQ, FU, CS, 384, KL_B384, false, -1, 0, -1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem); } while(0)
-			#define KL_ATTR(VF, HQ) do { KL_ATTR2(VF, HQ, true, false); KL_ATTR2(VF, HQ, false, false); KL_ATTR2(VF, HQ, false, true); } while(0)
-			KL_ATTR(false, false); KL_ATTR(true, false); KL_ATTR(true, true);
-			#undef KL_ATTR
-			#undef KL_ATTR2
-			cudaFuncSetAttribute(k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem);
-			cudaFuncSetAttribute(k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->kl_smem);
-		}
-	}
+	auto lp_atab = [d](const int32_t *taps, int ntaps) {                 // a low-pass of one k-step: the chroma's, SECAM's baseband
+		uint32_t ctab[256];
+		for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
+			ctab[(lo * 32 + lane) * 4 + reg] = kl_chroma_a_word(taps, ntaps, lane, reg, lo);
+		return((const uint32_t *) dev_copy(d, ctab, sizeof(ctab)));
+	};
+	if(p.path == PATH_LINE && dp.colour_mode != HTV_MONOCHROME) dt.chroma_atab = lp_atab(dp.chroma_taps, dp.chroma_ntaps);
+	if(p.ks) dt.sec_lpf_atab = lp_atab(dp.secam_lpf, 15);
 	if(secam)
 	{
-		const size_t rows = (size_t) d->sub_lines + 3;
 		const size_t groups = (size_t) (W + 2 + 7) / 8 + 1;
 		d->sec.rows = (int) rows;
 		{
@@ -2943,7 +3039,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			if(w && t->burst_win)
 			{
 				for(int x = dp.burst_left; x < W && x - dp.burst_left < t->burst_width; x++) w[x] = t->burst_win[x - dp.burst_left];
-				d->dt.sec_win = (const int16_t *) dev_copy(d, w, sizeof(int16_t) * W8);
+				dt.sec_win = (const int16_t *) dev_copy(d, w, sizeof(int16_t) * W8);
 			}
 			free(w);
 		}
@@ -2960,24 +3056,9 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		d->sec.iyc = (double *) dev_zero(d, sizeof(double) * ((size_t) W / SEC_IYC + 2) * rows);
 		d->sec.chk = (SecChk *) dev_zero(d, sizeof(SecChk) * rows);
 		d->sec.list = (int *) dev_zero(d, sizeof(int) * rows);
-		if(!d->sec.cbT || !d->sec.flags || !d->sec.yT || !d->sec.phT || !d->sec.iyc || !d->sec.chk || !d->sec.list || !d->sec.outc)
-		{
-			snprintf(err, errlen, "device allocation failed");
-			htv_dev_destroy(d);
-			return(NULL);
-		}
-		if(!d->dt.notch_atab && !(getenv("HTV_FIR") && !strcmp(getenv("HTV_FIR"), "scalar")))
-		{
-			uint32_t nt[MF_KSTEPS * 2 * 32 * 4];
-			for(int s3 = 0; s3 < MF_KSTEPS; s3++) for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
-				nt[((s3 * 2 + lo) * 32 + lane) * 4 + reg] = mf_a_word(dp.secam_notch, s3, lane, reg, lo);
-			d->dt.notch_atab = (const uint32_t *) dev_copy(d, nt, sizeof(nt));
-		}
-		const int W4s = (W + 3) & ~3;
-		const size_t sm = sizeof(int) * ((((W4s + 2 * LOFF + 14) + 3) & ~3) + W4s + 32) + 2 * (size_t) mf_row_bytes(W) + 32;
-		d->raster_smem = sm > d->raster_smem ? sm : d->raster_smem;
-		cudaFuncSetAttribute(k_raster_secam, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) d->raster_smem);
 	}
+	if(d->alloc_failed) return(create_fail(d, err, errlen, "device allocation failed"));
+	if(!plan_attributes(p, err, errlen)) { htv_dev_destroy(d); return(NULL); }
 	cudaEventCreate(&d->ev0);
 	cudaEventCreate(&d->ev1);
 	cudaStreamCreateWithFlags(&d->side, cudaStreamNonBlocking);
@@ -2992,16 +3073,12 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	cudaEventCreateWithFlags(&d->ev_r2, cudaEventDisableTiming);
 	cudaStreamCreateWithFlags(&d->side3, cudaStreamNonBlocking);
 	cudaEventCreateWithFlags(&d->ev_kl[1], cudaEventDisableTiming);
-	d->ahead = d->use_line && !(getenv("HTV_AHEAD") && !strcmp(getenv("HTV_AHEAD"), "0"));
+	d->ahead = p.path == PATH_LINE && !d->sw.no_ahead;
 	cudaEventCreateWithFlags(&d->ev_audio, cudaEventDisableTiming);
 	// the table build and the memsets above ran on the default stream, which the (non-blocking)
 	// streams the encoder works on do not wait for
 	if(cudaDeviceSynchronize() != cudaSuccess)
-	{
-		snprintf(err, errlen, "device initialisation failed (%s)", cudaGetErrorString(cudaGetLastError()));
-		htv_dev_destroy(d);
-		return(NULL);
-	}
+		return(create_fail(d, err, errlen, "device initialisation failed (%s)", cudaGetErrorString(cudaGetLastError())));
 	return(d);
 }
 
@@ -3213,7 +3290,7 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 		k_nicam_scan<<<1, 1024, 0, st>>>(d->dt, k_lo, k_hi);
 		d->launches += 2;
 		d->nic_kc = k_hi;                                          // fstart[k_hi] is valid; recompute from there next time
-		if(!d->use_line && !d->sec_line)
+		if(d->plan.path != PATH_LINE && d->plan.path != PATH_SEC_LINE)
 		{
 			// the split kernels' descriptor kernel (on `side`) reads both chains
 			CK(cudaEventRecord(d->ev_nic, d->side2));
@@ -3224,16 +3301,17 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	return(HTV_OK);
 }
 
-// The instantiation of the fused line kernel a launch uses, every template argument spelled out (htv_line_kernel); written
-// next to each launch, so that a change to the selection shows up in the name. The int16 forms keep their names; a store
-// that converts appends its sample type: ",ST=int8" compiled in, ",ST=-1:float" converting to dp.sample_type at run time.
-static void kl_name(char *s, size_t n, bool vf, bool hq, bool full, bool csat, int maxt, bool src, int snd, int wc,
-	int st = HTV_TYPE_INT16, int dyn_type = HTV_TYPE_INT16)
+// The plan's split modulator over n lines (htv_dev_render_lines, htv_dev_render_lines_rs): descriptors la, the composite
+// stream as k_raster / k_resample left it for this modulator (byte planes, int32, or the int16 `comp`), output o
+static void launch_mod(const htv_dev_t *d, int n, const LineAudio *la, const int16_t *comp, int16_t *o, const int16_t *acc,
+	int acc_rows, cudaStream_t st)
 {
-	char ts[24] = "";
-	if(st < 0) snprintf(ts, sizeof(ts), ",ST=-1:%s", htv_st_name(dyn_type));
-	else if(st != HTV_TYPE_INT16) snprintf(ts, sizeof(ts), ",ST=%s", htv_st_name(st));
-	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d%s>", vf, hq, full, csat, maxt, src, snd, wc, ts);
+	const DevPlan &p = d->plan;
+	const KMod &m = *p.mod;
+	const int grid = n < d->mod_grid ? n : d->mod_grid;                // the persistent forms
+	if(m.mma) m.mma<<<grid, p.line_threads, p.mod_smem, st>>>(d->dp, d->dt, la, d->d_planes, d->plane_stride, p.plane_pitch, n, o, acc, acc_rows);
+	else if(m.tma) m.tma<<<grid, p.line_threads, p.mod_smem, st>>>(d->dp, d->dt, la, d->d_comp32, n, o, acc, acc_rows);
+	else m.mod<<<n, p.line_threads, p.mod_smem, st>>>(d->dp, d->dt, la, comp, o, acc, acc_rows);
 }
 
 extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int16_t *d_out,
@@ -3241,6 +3319,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 {
 	DevGuard guard(d->device);
 	cudaStream_t st = (cudaStream_t) stream;
+	const DevPlan &p = d->plan;
 	if(nlines <= 0) return(HTV_OK);
 	// FM video with a pre-emphasis filter: the modulator also integrates the pipeline's fill line
 	const int fm_skip = d->dp.have_fmv && d->dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
@@ -3253,15 +3332,15 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		cudaFree(d->d_desc_r); cudaFree(d->d_desc_a); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
 		d->d_desc_r = d->d_desc_a = d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
 		d->desc_cap = 0;
-		if(d->use_line) CK(cudaMalloc(&d->d_desc_r2, 2 * sizeof(LineR2) * ((size_t) nlines + 2)));
+		if(p.path == PATH_LINE) CK(cudaMalloc(&d->d_desc_r2, 2 * sizeof(LineR2) * ((size_t) nlines + 2)));
 		else CK(cudaMalloc(&d->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 3)));
-		if(d->use_line || d->sec_line) CK(cudaMalloc(&d->d_desc_a2, 2 * sizeof(LineA2) * ((size_t) nlines + 1)));
-		if(d->ks_smem) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) nlines + 3)));
+		if(p.path == PATH_LINE || p.path == PATH_SEC_LINE) CK(cudaMalloc(&d->d_desc_a2, 2 * sizeof(LineA2) * ((size_t) nlines + 1)));
+		if(p.ks) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) nlines + 3)));
 		else CK(cudaMalloc(&d->d_desc_a, sizeof(LineAudio) * ((size_t) nlines + 1)));
 		d->desc_cap = nlines;
 	}
 	LineDescs ld = { (LineRaster *) d->d_desc_r + 1, (LineAudio *) d->d_desc_a };
-	if(d->use_line)
+	if(p.path == PATH_LINE)
 	{
 		// one persistent launch for the whole call: every CTA walks its own run of consecutive lines
 		const htv_dparams_t &dp = d->dp;
@@ -3304,34 +3383,8 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		if(run < 4) run = 4;
 		const int grid = (nlines + run - 1) / run;
 		if(d->timing) cudaEventRecord(d->ev0, st);
-		// another sample type than int16: the same forms with the store converting to dp.sample_type
-		const bool typed = dp.sample_type != HTV_TYPE_INT16;
-		#define KL_GO3(VF, HQ, FU, CS, T, B) do { \
-			kl_name(d->kname, sizeof(d->kname), VF, HQ, FU, CS, T, false, -1, 0, typed ? -1 : HTV_TYPE_INT16, dp.sample_type); \
-			if(typed) k_line<VF, HQ, FU, CS, T, B, false, -1, 0, -1><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); \
-			else k_line<VF, HQ, FU, CS, T, B><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0); } while(0)
-		#define KL_GO2(VF, HQ, FU, CS) do { \
-			if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, CS, 256, KL_B256); \
-			else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, CS, 320, KL_B320); \
-			else KL_GO3(VF, HQ, FU, CS, 384, KL_B384); } while(0)
-		// the common case (128 | W, a chroma filter that cannot overflow) gets its own instantiation; everything else the general one
-		#define KL_GO(VF, HQ) do { if(dp.W % MF_TILE == 0 && !d->kl_csat) KL_GO2(VF, HQ, true, false); \
-			else if(!d->kl_csat) KL_GO2(VF, HQ, false, false); else KL_GO2(VF, HQ, false, true); } while(0)
-		if(!dp.vf_type) KL_GO(false, false);
-		// ... and within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those sound stages
-		// and the width compiled in, storing int16 or int8 (the HackRF's format); other sample types run the general form
-		else if(dp.vf_type == 3 && !d->kl_csat && dp.W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !d->kl_general &&
-			(dp.sample_type == HTV_TYPE_INT16 || dp.sample_type == HTV_TYPE_INT8))
-		{
-			kl_name(d->kname, sizeof(d->kname), true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, dp.sample_type);
-			if(typed) k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
-			else k_line<true, true, true, false, 256, KL_B256, false, KL_SND_FM_NICAM, 1024><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0);
-		}
-		else if(dp.vf_type == 3) KL_GO(true, true);
-		else KL_GO(true, false);
-		#undef KL_GO
-		#undef KL_GO2
-		#undef KL_GO3
+		strcpy(d->kname, p.kname);
+		p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0, NULL);
 		CK(cudaEventRecord(d->ev_kl[buf], st));
 		d->launches += 4;
 		d->last_mod_lines = nlines;
@@ -3341,14 +3394,14 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		CK(cudaGetLastError());
 		return(HTV_OK);
 	}
-	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, ld, line0, nlines, d->ks_smem ? (LineS2 *) d->d_desc_s2 : NULL);
+	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, ld, line0, nlines, p.ks ? (LineS2 *) d->d_desc_s2 : NULL);
 	if(!d->side_armed)
 	{
 		CK(cudaEventRecord(d->ev_in, st));
 		CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
 	}
 	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
-	if(d->sec_line)
+	if(p.path == PATH_SEC_LINE)
 	{
 		// the sound descriptors of the fused line kernel, each half on the side stream of the pre-pass chain it depends on
 		const int dgrid = (nlines + KD_LINES * KD_WARPS - 1) / (KD_LINES * KD_WARPS);
@@ -3363,23 +3416,20 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 	d->launches += 2;
 	d->side_armed = 0;
 	bool joined = false;
-	const bool typed = d->dp.sample_type != HTV_TYPE_INT16;         // the modulators' store converts (post_store<true>)
 	for(int done = 0; done < nlines; done += d->sub_lines)
 	{
 		const int n = nlines - done < d->sub_lines ? nlines - done : d->sub_lines;
 		const bool last = done + n >= nlines;
 		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * d->dp.W * htv_st_bytes(d->dp.sample_type, d->dp.complex_out));
-		const int16_t *sadd = NULL;
 		const int16_t *cstream = d->d_comp;
 		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * d->dp.W * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
-		char rname[64], mname[128];                   // raster and modulator kernels of this sub-batch (htv_line_kernel)
 		if(d->dp.colour_mode == HTV_SECAM)
 		{
 			// rows 0 .. n+2 <-> lines first-2 .. first+n; the chain covers rows 0 .. n+1
 			const LineRaster *lr = ld.r + done - 1;
-			if(d->ks_smem)
+			if(p.ks)
 			{
 				// rows 0 .. n+2: their own compact descriptors, then runs of rows per persistent CTA
 				const LineS2 *ls = (const LineS2 *) d->d_desc_s2 + done;
@@ -3387,30 +3437,16 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				int run = (nr + d->kl_ctas - 1) / d->kl_ctas;
 				if(run < 4) run = 4;
 				const int grid = (nr + run - 1) / run;
-				const bool full = d->dp.W % MF_TILE == 0;
-				#define KS_GO2(FU, T, B) do { \
-					snprintf(rname, sizeof(rname), "k_sec_raster<FULL=%d,MAXT=%d>", FU, T); \
-					k_sec_raster<FU, T, B><<<grid, d->kl_threads, d->ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec); } while(0)
-				#define KS_GO(FU) do { \
-					if(d->kl_threads <= 256) KS_GO2(FU, 256, KL_B256); \
-					else if(d->kl_threads <= 320) KS_GO2(FU, 320, KL_B320); \
-					else KS_GO2(FU, 384, KL_B384); } while(0)
-				if(full) KS_GO(true); else KS_GO(false);
-				#undef KS_GO
-				#undef KS_GO2
+				p.ks->fn<<<grid, p.kl_threads, p.ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec);
 				d->launches++;
 			}
-			else
-			{
-				snprintf(rname, sizeof(rname), "k_raster_secam");
-				k_raster_secam<<<n + 3, d->line_threads, d->raster_smem, st>>>(d->dp, d->dt, lr, d->d_comp, d->sec);
-			}
+			else k_raster_secam<<<n + 3, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, lr, d->d_comp, d->sec);
 			// the chain (htv_secam.cuh): pass 0 over every line, the predictor, then refinement passes until no line's
 			// outgoing state changes - at that fixed point every line was computed from its true predecessor state =
 			// the sequential result. The loop needs the change count on the host, so SECAM launches synchronise.
 			const int nch = n + 2, nb = (nch + 31) / 32;
 			cudaEvent_t dbg0 = NULL, dbg1 = NULL;
-			const bool dbg = getenv("HTV_DEBUG") != NULL;
+			const bool dbg = d->sw.debug;
 			if(dbg) { cudaEventCreate(&dbg0); cudaEventCreate(&dbg1); cudaEventRecord(dbg0, st); }
 			int pass = 0, changed = 1, repredict = d->sec_repredict;
 			htv_secam_chain_t &cs = d->sec_stats;
@@ -3478,72 +3514,35 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		else
 		{
 			// raster lines done-1 .. done+n (descriptor index = line - (line0 - 1))
-			snprintf(rname, sizeof(rname), "k_raster");
-			k_raster<<<n + 2, d->line_threads, d->raster_smem, st>>>(d->dp, d->dt, ld.r + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, d->plane_pitch);
+			k_raster<<<n + 2, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, ld.r + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, p.plane_pitch);
 			d->launches++;
 		}
 		if(!joined)
 		{
 			CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
-			if(d->sec_line) CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
+			if(p.path == PATH_SEC_LINE) CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
 			joined = true;
 		}
 		if(d->timing && last) cudaEventRecord(d->ev0, st);
-		if(d->dp.have_fmv)
+		if(p.path == PATH_FMV)
 		{
 			const int pre = fm_skip && done == 0 ? 1 : 0, rows = n + pre;
 			const LineAudio *lap = ld.a + done + fm_skip - pre;
-			const htv_dparams_t &dp = d->dp;
-			if(dp.fmv_ntaps == 67) k_fmv_base<67><<<rows, d->line_threads, d->fmv_smem, st>>>(dp, d->dt, lap, cstream, sadd, pre);
-			else if(dp.fmv_ntaps == 71) k_fmv_base<71><<<rows, d->line_threads, d->fmv_smem, st>>>(dp, d->dt, lap, cstream, sadd, pre);
-			else if(dp.fmv_ntaps == 0) k_fmv_base<0><<<rows, d->line_threads, d->fmv_smem, st>>>(dp, d->dt, lap, cstream, sadd, pre);
-			else { fprintf(stderr, "hacktv_b200: unsupported FM pre-emphasis length %d\n", dp.fmv_ntaps); return(HTV_ERROR); }
+			p.fmv_base->fn<<<rows, p.line_threads, p.fmv_smem, st>>>(d->dp, d->dt, lap, cstream, pre);
 			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, rows);
-			if(typed) k_fmv_mod<true><<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
-			else k_fmv_mod<false><<<rows, d->line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
-			snprintf(mname, sizeof(mname), "k_fmv_base<%d> + k_fmv_scan + k_fmv_mod", dp.fmv_ntaps);
+			p.fmv_mod->fn<<<rows, p.line_threads, 0, st>>>(d->dp, d->dt, lap, o, acc, acc_rows, -pre);
 			d->launches += 2;
 		}
-		else if(d->sec_line)
+		else if(p.path == PATH_SEC_LINE)
 		{
 			// runs of at least 4 lines (every run stages two lines more than it emits)
-			const htv_dparams_t &dp = d->dp;
 			int run = (n + d->kl_ctas - 1) / d->kl_ctas;
 			if(run < 4) run = 4;
 			const int grid = (n + run - 1) / run;
-			#define KL_GO3(VF, HQ, FU, T, B) do { \
-				kl_name(mname, sizeof(mname), VF, HQ, FU, false, T, true, -1, 0, typed ? -1 : HTV_TYPE_INT16, dp.sample_type); \
-				if(typed) k_line<VF, HQ, FU, false, T, B, true, -1, 0, -1><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); \
-				else k_line<VF, HQ, FU, false, T, B, true><<<grid, d->kl_threads, d->kl_smem, st>>>(dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp); } while(0)
-			#define KL_GO2(VF, HQ, FU) do { \
-				if(d->kl_threads <= 256) KL_GO3(VF, HQ, FU, 256, KL_B256); \
-				else if(d->kl_threads <= 320) KL_GO3(VF, HQ, FU, 320, KL_B320); \
-				else KL_GO3(VF, HQ, FU, 384, KL_B384); } while(0)
-			#define KL_GO(VF, HQ) do { if(dp.W % MF_TILE == 0) KL_GO2(VF, HQ, true); else KL_GO2(VF, HQ, false); } while(0)
-			if(!dp.vf_type) KL_GO(false, false);
-			else if(dp.vf_type == 3) KL_GO(true, true);
-			else KL_GO(true, false);
-			#undef KL_GO
-			#undef KL_GO2
-			#undef KL_GO3
+			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(d->dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp);
 		}
-		else if(d->d_planes)
-		{
-			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_mma<256,4>"); { if(typed) k_mod_mma<256, 4, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); else k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); } }
-			else { snprintf(mname, sizeof(mname), "k_mod_mma<384,2>"); { if(typed) k_mod_mma<384, 2, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_planes, d->plane_stride, d->plane_pitch, n, o, acc, acc_rows); } }
-		}
-		else if(d->d_comp32)
-		{
-			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod_tma<256,4>"); { if(typed) k_mod_tma<256, 4, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); } }
-			else { snprintf(mname, sizeof(mname), "k_mod_tma<384,2>"); { if(typed) k_mod_tma<384, 2, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, ld.a + done, d->d_comp32, n, o, acc, acc_rows); } }
-		}
-		else if(d->line_threads <= 256) { snprintf(mname, sizeof(mname), "k_mod<256,4>"); { if(typed) k_mod<256, 4, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); else k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); } }
-		else { snprintf(mname, sizeof(mname), "k_mod<384,2>"); { if(typed) k_mod<384, 2, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, ld.a + done, cstream, sadd, o, acc, acc_rows); } }
-		// a modulator whose store converts: its template argument TY, with the type (k_line spells its own)
-		snprintf(d->kname, sizeof(d->kname), "%s + %s%s%s", rname, mname, typed && !d->sec_line ? " ST=-1:" : "",
-			typed && !d->sec_line ? htv_st_name(d->dp.sample_type) : "");
+		else launch_mod(d, n, ld.a + done, cstream, o, acc, acc_rows, st);
+		strcpy(d->kname, p.kname);
 		d->launches++;
 		if(last) d->last_mod_lines = n;
 	}
@@ -3601,7 +3600,8 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	DevGuard guard(d->device);
 	cudaStream_t st = (cudaStream_t) stream;
 	if(nlines <= 0) return(HTV_OK);
-	if(!d->d_rs_taps || d->plane_pitch || d->dp.have_fmv || r->dp.colour_mode == HTV_SECAM || (d->dp.W & 3)) return(HTV_ERROR);
+	const DevPlan &p = d->plan;
+	if(p.path != PATH_RS || r->plan.path != PATH_RASTER || p.plane_pitch || (d->dp.W & 3)) return(HTV_ERROR);
 	if(nlines > d->desc_cap)
 	{
 		cudaStreamSynchronize(st);
@@ -3637,7 +3637,6 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	CK(cudaEventRecord(d->ev_audio, d->side));
 	d->side_armed = 0;
 	bool joined = false;
-	const bool typed = d->dp.sample_type != HTV_TYPE_INT16;         // the modulators' store converts (post_store<true>)
 	d->launches += 2;
 	const int Ws = d->dp.W, Wp = r->dp.W;
 	int sub = d->sub_lines < r->sub_lines ? d->sub_lines : r->sub_lines;
@@ -3649,30 +3648,16 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * Ws * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
 		// raster lines line0 + done - 1 .. line0 + done + n + 1 -> rows 0 .. n + 2 of the raster context's int16 stream
-		k_raster<<<n + 3, r->line_threads, r->raster_smem, st>>>(r->dp, r->dt, ldr.r + done, r->d_comp, NULL, NULL, 0, 0);
+		k_raster<<<n + 3, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt, ldr.r + done, r->d_comp, NULL, NULL, 0, 0);
 		// resampled lines line0 + done .. line0 + done + n + 1 -> rows 0 .. n + 1 of this context's scratch
-		k_resample<<<n + 2, d->line_threads, 0, st>>>(r->d_comp, Wp, Ws, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
-			d->d_planes, d->plane_stride, d->d_planes ? NULL : d->d_comp32, d->d_comp);
+		k_resample<<<n + 2, p.line_threads, 0, st>>>(r->d_comp, Wp, Ws, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
+			d->d_planes, d->plane_stride, d->d_comp32, d->d_comp);
 		d->launches += 2;
 		if(!joined) { CK(cudaStreamWaitEvent(st, d->ev_audio, 0)); joined = true; }
 		if(d->timing && last) cudaEventRecord(d->ev0, st);
-		if(d->d_planes)
-		{
-			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { if(typed) k_mod_mma<256, 4, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); else k_mod_mma<256, 4><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); }
-			else { if(typed) k_mod_mma<384, 2, true><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); else k_mod_mma<384, 2><<<grid, d->line_threads, d->modm_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_planes, d->plane_stride, 0, n, o, acc, acc_rows); }
-		}
-		else if(d->d_comp32)
-		{
-			const int grid = n < d->mod_grid ? n : d->mod_grid;
-			if(d->line_threads <= 256) { if(typed) k_mod_tma<256, 4, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<256, 4><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); }
-			else { if(typed) k_mod_tma<384, 2, true><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); else k_mod_tma<384, 2><<<grid, d->line_threads, d->modt_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp32, n, o, acc, acc_rows); }
-		}
-		else if(d->line_threads <= 256) { if(typed) k_mod<256, 4, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); else k_mod<256, 4><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); }
-		else { if(typed) k_mod<384, 2, true><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); else k_mod<384, 2><<<n, d->line_threads, d->mod_smem, st>>>(d->dp, d->dt, lda.a + done, d->d_comp, NULL, o, acc, acc_rows); }
+		launch_mod(d, n, lda.a + done, d->d_comp, o, acc, acc_rows, st);
 		d->launches++;
-		snprintf(d->kname, sizeof(d->kname), "k_raster + k_resample + %s<%d,%d>%s%s", d->d_planes ? "k_mod_mma" : d->d_comp32 ? "k_mod_tma" : "k_mod",
-			d->line_threads <= 256 ? 256 : 384, d->line_threads <= 256 ? 4 : 2, typed ? " ST=-1:" : "", typed ? htv_st_name(d->dp.sample_type) : "");
+		strcpy(d->kname, p.kname);
 		if(last) d->last_mod_lines = n;
 	}
 	if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
@@ -3725,8 +3710,19 @@ extern "C" int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalu
 	return(HTV_OK);
 }
 
-// The sample type the stores convert to (htv_set_sample_type): read from dp at every launch
-extern "C" void htv_dev_set_sample_type(htv_dev_t *d, int type) { d->dp.sample_type = type; }
+// The sample type the stores convert to (htv_set_sample_type, before the first rendered line): the plan again, for the
+// instantiations whose store converts
+extern "C" int htv_dev_set_sample_type(htv_dev_t *d, int type)
+{
+	DevGuard guard(d->device);
+	DevPlan p;
+	char err[256];
+	const bool ok = plan_kernels(d->tab, d->sw, type, &p, err, sizeof(err)) == HTV_OK && plan_attributes(p, err, sizeof(err));
+	if(!ok) { fprintf(stderr, "hacktv_b200: %s\n", err); return(HTV_ERROR); }
+	d->plan = p;
+	d->dp.sample_type = type;
+	return(HTV_OK);
+}
 
 // htv_convert: dst[i] = the `type` form of src[i] (htv_sample_type.h), eight values per thread and step: one 16-byte
 // load, one store of 8, 16 or 32 bytes

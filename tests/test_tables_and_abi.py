@@ -225,3 +225,57 @@ def test_line_width_matrix_covers_every_instantiation(built):
     ran = {FIXED} | {part for c in MATRIX for part in c[4].split(" + ")}
     assert not want - ran, sorted(want - ran)
     assert not ran - want, sorted(ran - want)
+
+
+def _plan_name(H, mode, rate, kw, prate=0, sample_type="int16", **env):
+    """htv_dev_plan_name: the line kernel(s) the C selection (plan_kernels in htv_kernels.cu, the code htv_dev_create
+    runs) picks for an encoder of these tables writing this sample type, under the switches in `env`. No GPU needed."""
+    from test_gpu_zz_line_widths import _env
+    L = H.lib()
+    L.htv_dev_plan_name.restype = C.c_int
+    L.htv_dev_plan_name.argtypes = [C.c_void_p, C.c_int, C.c_char_p, C.c_size_t]
+    t = H.Tables(H.mode_config(mode, **kw), rate, prate)
+    buf = C.create_string_buffer(256)
+    with _env(**env):
+        r = L.htv_dev_plan_name(t._t, H.SAMPLE_TYPES[sample_type], buf, len(buf))
+    t.close()
+    assert r == H.HTV_OK, buf.value.decode()
+    return buf.value.decode()
+
+
+def test_c_selection_runs_what_the_line_width_matrix_asserts(built):
+    """The C selection itself names, for every case of the GPU line-width matrix, the instantiation the case asserts the
+    encoder ran; so does it for the form with PAL's sound stages compiled in, and the general form under HTV_KL=general."""
+    from test_gpu_zz_line_widths import FIXED, GENERAL, MATRIX
+    for mode, rate, kw, _, kernel in MATRIX:
+        assert _plan_name(built, mode, rate, kw) == kernel, (mode, rate, kw)
+    for mode in ("i", "b"):
+        assert _plan_name(built, mode, 16000000, dict(vfilter=True)) == FIXED
+        assert _plan_name(built, mode, 16000000, dict(vfilter=True), HTV_KL="general") == GENERAL
+
+
+def test_c_selection_runs_what_the_sample_type_cases_assert(built):
+    """Every case of the GPU sample-type test, for each type: the names it asserts (the split modulators, FM video and
+    --pixelrate among them), and the int8 form with PAL's sound stages compiled in, or the general one under HTV_KL=general."""
+    from test_gpu_zz_sample_types import CASES, FIXED_INT8, TYPES
+    for case, (mode, rate, prate, kw, env, _, kernel) in sorted(CASES.items()):
+        for st in TYPES:
+            name = _plan_name(built, mode, rate, kw, prate, st, **env)
+            want = FIXED_INT8 if st == "int8" and case in ("i-16M-filter", "i-16M-filter-passthru") else kernel
+            assert want.format(st=st) in name, (case, st, name)
+            if "k_line" in want:
+                assert name == want.format(st=st), (case, st, name)
+            else:
+                assert f"ST=-1:{st}" in name, (case, st, name)
+    assert _plan_name(built, "i", 16000000, dict(vfilter=True), sample_type="int8") == FIXED_INT8
+    assert _plan_name(built, "i", 16000000, dict(vfilter=True), sample_type="int8", HTV_KL="general") == \
+        "k_line<VF=1,HQ=1,FULL=1,CSAT=0,MAXT=256,SRC=0,SND=-1,WC=0,ST=-1:int8>"
+
+
+def test_c_selection_of_the_scalar_video_filter(built):
+    """HTV_FIR=scalar: PAL-I falls back to the split kernels with the TMA-fed modulator, SECAM keeps k_line<SRC> behind
+    the raster with the scalar notch."""
+    F = dict(vfilter=True)
+    assert _plan_name(built, "i", 16000000, F, HTV_FIR="scalar") == "k_raster + k_mod_tma<256,4>"
+    assert _plan_name(built, "l", 16000000, F, HTV_FIR="scalar") == \
+        "k_raster_secam + k_line<VF=1,HQ=1,FULL=1,CSAT=0,MAXT=256,SRC=1,SND=-1,WC=0>"
