@@ -36,8 +36,6 @@
 #define RS (1 << RS_BITS)             // NICAM symbol ring
 #define RF_BITS 14
 #define RF (1 << RF_BITS)             // NICAM frame ring
-#define MAX_SEG 8                     // audio samples overlapping one scan line (+1)
-#define MAX_NSYM 64                   // NICAM symbols overlapping one scan line
 
 #define CK(x) do { cudaError_t e_ = (x); if(e_ != cudaSuccess) { \
 	fprintf(stderr, "hacktv_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return(HTV_ERROR); } } while(0)
@@ -217,8 +215,9 @@ struct htv_dev_t {
 	int r2_armed;
 	int side_armed;
 	int ev_pending;
-	void *d_desc_r, *d_desc_a;        // LineRaster[cap + 2], LineAudio[cap]
-	void *d_desc_r2, *d_desc_a2;      // LineR2[cap + 2], LineA2[cap] (fused line kernel)
+	void *d_desc_r;                   // LineRaster[cap + 2]
+	void *d_desc_r2;                  // LineR2[cap + 2] x 2 (fused line kernel)
+	void *d_desc_a2;                  // LineA2[cap + 1] (x 2 for the fused line kernel)
 	void *d_desc_s2;                  // LineS2[cap + 3] (SECAM raster in the fused kernel's form)
 	int desc_cap;
 	int kl_ctas;                      // persistent CTAs of the fused kernels (k_line, k_sec_raster)
@@ -633,20 +632,7 @@ struct __align__(16) LineRaster {
 	int ov_any, pad2;
 };
 
-// Sound-carrier state at the start of a line
-struct __align__(16) LineAudio {
-	long long m0;                     // audio-clock index of the line's first sample
-	unsigned long long am_phase0, off_phase0;
-	unsigned long long seg_phase[MAX_SEGS], seg_ang[MAX_SEGS];
-	int seg_x[MAX_SEGS + 1];          // first sample (relative to the line) of each audio segment
-	int seg_am[MAX_SEGS];
-	int nseg, kk0, cc0, nsym;
-	int symrow[MAX_SYMS];             // pulse-table rows: I row | Q row << 16, or -1 (use the generic sum)
-	int sym[MAX_SYMS];                // per symbol: first sample relative to the line (x4, arithmetic), bit 0: I polarity +, bit 1: Q polarity +
-	int pad1[2];
-};
-
-// Sound-carrier state of a line for the fused line kernel (htv_line.cuh), built by k_line_desc_a2 (one warp per line)
+// Sound-carrier state of a line for the sound stage (htv_sound.cuh), built by k_line_desc_a2 (one warp per line)
 struct __align__(16) LineA2 {
 	unsigned long long seg_phase[MAX_SEGS], seg_ang[MAX_SEGS];   // FM phase at the line's sample 0 / per sample, per audio segment
 	unsigned long long am_phase0, off_phase0;
@@ -665,8 +651,6 @@ struct __align__(16) LineA2 {
 	int pad[2];
 };
 
-struct LineDescs { LineRaster *r; LineAudio *a; };
-
 // What the raster half needs to know about a line (64 bytes, read through the read-only path)
 struct __align__(16) LineR2 {
 	int valid;                        // 0: before the stream
@@ -682,7 +666,7 @@ struct __align__(16) LineR2 {
 };
 static_assert(sizeof(LineR2) == 64, "LineR2 is read as four int4");
 
-static_assert(sizeof(LineRaster) % 16 == 0 && sizeof(LineAudio) % 16 == 0 && sizeof(LineA2) % 16 == 0, "descriptors are copied as int4");
+static_assert(sizeof(LineRaster) % 16 == 0 && sizeof(LineA2) % 16 == 0, "descriptors are copied as int4");
 
 // frame / line / picture row of scan line L; L < 0 are the pipeline-fill lines the reference's
 // SECAM stage sees before line 1 (frame 1, line 0: an all-black active line, ref video.c:4665-4667)
@@ -814,91 +798,11 @@ __device__ void line_raster(const htv_dparams_t &dp, const DevTables &dt, int64_
 	li.nent = n;
 }
 
-__device__ void line_audio(const htv_dparams_t &dp, const DevTables &dt, int64_t L, LineAudio &la)
-{
-	const int W = dp.W;
-	const int64_t m0 = L * (int64_t) W + dp.shift;
-	la.m0 = m0;
-	la.kk0 = (int) (m0 % 32767);
-	la.cc0 = dp.have_nicam ? (int) (m0 % dp.nicam_cc_len) : 0;
-	la.am_phase0 = dp.am_ang * (unsigned long long) m0;
-	la.off_phase0 = dp.offset_phase0 + dp.offset_ang * (unsigned long long) (m0 - 32767);
-	// audio segments: audio index j is in effect from seg_start(j) up to seg_start(j + 1)
-	int n = 0;
-	if(dp.have_fm || dp.have_am)
-	{
-		int64_t j = fetches_by(m0, dp.rate) - 1;
-		for(; n < MAX_SEGS; n++, j++)
-		{
-			const int64_t st = seg_start(j, dp.rate);
-			if(st >= m0 + W) break;
-			la.seg_x[n] = (int) max((int64_t) 0, st - m0);
-			la.seg_phase[n] = 0; la.seg_ang[n] = 0;
-			if(dp.have_fm)
-			{
-				const unsigned long long ang = dt.fm_ang[(int) dt.fm_p[(j + 1) & (RA - 1)] + 32768];
-				// phase at relative sample x = B(j) + (m0 + x - st + 1) * ang
-				la.seg_ang[n] = ang;
-				la.seg_phase[n] = dt.fm_B[(j + 1) & (RA - 1)] + ang * (unsigned long long) (m0 - st + 1);
-			}
-			la.seg_am[n] = dp.have_am ? pcm_mono(dt, j, dp.volume) : 0;
-		}
-	}
-	la.nseg = n;
-	for(int i = n; i <= MAX_SEGS; i++) la.seg_x[i] = 0x7FFFFFFF;
-	la.nsym = 0;
-	if(dp.have_nicam)
-	{
-		// symbols whose pulse can still reach this line: ntaps samples back
-		const int64_t sfirst = (int64_t) (((unsigned long long) max((int64_t) 0, m0 - dp.nicam_ntaps) * dp.nicam_D) / dp.nicam_F);
-		const int64_t slast = (int64_t) (((unsigned long long) (m0 + W - 1) * dp.nicam_D) / dp.nicam_F);
-		const int ns = (int) min((int64_t) MAX_SYMS, slast - sfirst + 1);
-		// walk the symbols incrementally: pos = ceil(s * F / D), rem = pos * D - s * F. Start 5
-		// symbols early to know the polarities / spacings behind the first listed one.
-		const int lead = (int) min((int64_t) 5, sfirst);
-		int64_t s = sfirst - lead, k = s / 364, pos = nic_sym_pos(s, dp.nicam_F, dp.nicam_D);
-		int ks = (int) (s - k * 364);
-		int rem = (int) (pos * dp.nicam_D - s * dp.nicam_F);
-		int fst = dt.nic_fstart[k & (RF - 1)];
-		int patI = 0, patQ = 0, gaps = 0, prev_adv = 0;
-		for(int i = -lead; i < ns; i++)
-		{
-			const int sy = (fst + dt.nic_local[s & (RS - 1)]) & 3;
-			// ref nicam728.c:47,386-391: _syms = {0,1,3,2}; bit0 -> I polarity, bit1 -> Q polarity
-			const int code = sy == 2 ? 3 : (sy == 3 ? 2 : sy);
-			patI = ((patI << 1) | (code & 1)) & 63;
-			patQ = ((patQ << 1) | ((code >> 1) & 1)) & 63;
-			if(i > -lead || s > 0)
-			{
-				const int minor = dp.nicam_minor_short ? prev_adv == dp.nicam_sps - 1 : prev_adv == dp.nicam_sps;
-				gaps = ((gaps << 1) | (s > 0 ? minor : 0)) & 31;
-			}
-			if(i >= 0)
-			{
-				la.sym[i] = (int) ((pos - m0) * 4) | (code & 3);
-				int row = -1;
-				if(dp.nicam_lut_ok && s >= 5 && __popc(gaps) <= 1)
-				{
-					const int g = gaps ? 1 + (31 - __clz(gaps & -gaps)) : 0;   // which gap (1 = newest) has the rarer spacing
-					row = (g * 64 + patI) | ((g * 64 + patQ) << 16);
-				}
-				la.symrow[i] = row;
-			}
-			const int adv = (dp.nicam_F - rem + dp.nicam_D - 1) / dp.nicam_D;
-			pos += adv; rem += adv * dp.nicam_D - dp.nicam_F;
-			prev_adv = adv;
-			s++;
-			if(++ks == 364) { ks = 0; k++; fst = dt.nic_fstart[k & (RF - 1)]; }
-		}
-		la.nsym = ns;
-	}
-}
-
 // ---------------------------------------------------------------------------
-// Sound descriptors for the fused line kernel: ONE WARP per scan line. The same closed forms as
-// line_audio() (one thread per line, a serial walk over ~30 symbols), spread over the lanes: lane = audio
-// segment, lane = NICAM symbol, lane = 32-sample block. 64-bit divisions by run-time constants go
-// through fp64 (exact below 2^52, with the exact division behind it).
+// Sound descriptors (LineA2) for every modulator: ONE WARP per scan line. The closed forms of the sound
+// carriers' state at the line's start, spread over the lanes: lane = audio segment, lane = NICAM symbol,
+// lane = 32-sample block. 64-bit divisions by run-time constants go through fp64 (exact below 2^52, with
+// the exact division behind it).
 // ---------------------------------------------------------------------------
 
 // floor(n / d) and the remainder for n < 2^63, 0 < d < 2^31
@@ -1100,7 +1004,7 @@ k_line_desc_a2(const __grid_constant__ htv_dparams_t dp, const DevTables dt, Lin
 			const int patI = (int) (__brev(wi) >> 26), patQ = (int) (__brev(wq) >> 26), gaps = (int) (__brev(wg) >> 27);
 			const int sx = dq + (int) p;
 			int bI = 0xFFFF, bQ = 0xFFFF;
-			// a row needs the 5 predecessors inside the window (and, as in line_audio, a stream that is 5 symbols old)
+			// a row needs the 5 predecessors inside the window (and a stream that is 5 symbols old)
 			const bool row_ok = dp.nicam_lut_ok && i >= 5 && s0 + i >= 5 && __popc(gaps) <= 1;
 			if(row_ok)
 			{
@@ -1172,12 +1076,12 @@ __device__ __forceinline__ void line_s2(const htv_dparams_t &dp, const DevTables
 }
 
 // s2 (SECAM with k_sec_raster): the same lines once more in that kernel's compact form, s2[i] <-> line line0 - 2 + i
-__global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const DevTables dt, LineDescs ld, int64_t line0, int nlines, LineS2 *s2)
+__global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const DevTables dt, LineRaster *lr, int64_t line0, int nlines, LineS2 *s2)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if(i >= nlines + 3) return;
-	line_raster(dp, dt, line0 - 2 + i, ld.r[i - 1]);
-	if(s2) line_s2(dp, dt, line0 - 2 + i, ld.r[i - 1], s2[i]);
+	line_raster(dp, dt, line0 - 2 + i, lr[i - 1]);
+	if(s2) line_s2(dp, dt, line0 - 2 + i, lr[i - 1], s2[i]);
 }
 
 // the same for the fused line kernel (htv_line.cuh): compact descriptors, index 0 .. nlines+1 <-> line line0-1 .. line0+nlines
@@ -1198,14 +1102,6 @@ __global__ void k_line_desc_r2(const __grid_constant__ htv_dparams_t dp, const D
 	o.row_off = li.row_off;
 	o.pad = 0;
 	out[i] = o;
-}
-
-// sound-carrier descriptors for lines line0 .. line0+nlines-1 (needs the audio pre-pass results)
-__global__ void k_line_desc_a(const __grid_constant__ htv_dparams_t dp, const DevTables dt, LineDescs ld, int64_t line0, int nlines)
-{
-	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if(i >= nlines) return;
-	line_audio(dp, dt, line0 + i, ld.a[i]);
 }
 
 __device__ __forceinline__ int round_away(double v)
@@ -1742,181 +1638,17 @@ __global__ void __launch_bounds__(256) k_overlay_secam(const __grid_constant__ h
 // and writes int16 IQ with 128-bit streaming stores.
 // ---------------------------------------------------------------------------
 
-// Everything k_mod does for 4 consecutive samples once the composite window is in shared
-// memory. cwin[j] = composite sample x0 - 25 - CSKEW + j (16-byte aligned).
-// The sound carriers of 4 consecutive samples, added into oi/oq (ref video.c:3261-3450,
-// nicam728.c:342-411). Shared by the AM/VSB modulator and the FM-video baseband kernel.
-// PRECISE (FM video only): the carrier is evaluated in fp64 from the full 64-bit phase. An FM
-// modulator integrates its input, so a sound-carrier sample that is 1 LSB off turns everything
-// after it; the fast fp32 evaluation loses the sign of a carrier sample that lands on a zero
-// crossing (an unmodulated 6.5 MHz carrier at 20 Msps does so every 40 samples).
-template<bool PRECISE>
-__device__ __forceinline__ void sound_add(const htv_dparams_t &dp, const DevTables &dt, const LineAudio &la,
-	const short *ntp, int x0, int (&oi)[SPT], int (&oq)[SPT])
-{
-	if(dp.have_fm || dp.have_am)
-	{
-		// at most one audio-sample boundary falls inside 4 consecutive samples
-		int sg0 = 0;
-		while(la.seg_x[sg0 + 1] <= x0) sg0++;
-		const int nb = la.seg_x[sg0 + 1];
-		const int sg1 = min(sg0 + 1, MAX_SEGS - 1);
-		const unsigned long long angA = la.seg_ang[sg0], angB = la.seg_ang[sg1];
-		unsigned long long phA = la.seg_phase[sg0] + angA * (unsigned long long) x0;
-		unsigned long long phB = la.seg_phase[sg1] + angB * (unsigned long long) x0;
-		unsigned long long phM = la.am_phase0 + dp.am_ang * (unsigned long long) (x0 + 1);
-		const int amA = (la.seg_am[sg0] + 32768) / 2, amB = (la.seg_am[sg1] + 32768) / 2;
-		int kk = la.kk0 + x0; if(kk >= 32767) kk -= 32767;
-		#pragma unroll
-		for(int k = 0; k < SPT; k++, kk++)
-		{
-			const bool second = x0 + k >= nb;
-			if(kk >= 32767) kk -= 32767;
-			// amplitude of the reference's Q31 phasor kk+1 multiplications after a renormalisation
-			const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
-			if(dp.have_fm)
-			{
-				const unsigned long long ph = second ? phB : phA;
-				if(PRECISE)
-				{
-					double sn, cs;
-					sincospi((double) (long long) ph * 1.0842021724855044e-19, &sn, &cs);     // 2 / 2^64
-					const double ampd = 32767.999984741211 - (double) (kk + 1) * 1.52587890625e-5;
-					oi[k] += (min((int) floor(ampd * cs), 32767) * dp.fm_level) >> 15;
-					oq[k] += (min((int) floor(ampd * sn), 32767) * dp.fm_level) >> 15;
-				}
-				else
-				{
-					float sn, cs;
-					__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);   // pi / 2^31
-					oi[k] += ((int) floorf(amp * cs) * dp.fm_level) >> 15;
-					oq[k] += ((int) floorf(amp * sn) * dp.fm_level) >> 15;
-				}
-				phA += angA; phB += angB;
-			}
-			if(dp.have_am)
-			{
-				float sn, cs;
-				__sincosf((float) (int) (phM >> 32) * 1.4629180792671596e-9f, &sn, &cs);
-				const int smp = second ? amB : amA;
-				oi[k] += ((((int) floorf(amp * cs) * smp) >> 15) * dp.am_level) >> 15;
-				oq[k] += ((((int) floorf(amp * sn) * smp) >> 15) * dp.am_level) >> 15;
-				phM += dp.am_ang;
-			}
-		}
-	}
+#include "htv_sound.cuh"
 
-	if(dp.have_nicam)
-	{
-		// the newest symbol started at or before the thread's last sample: estimate from the
-		// mean spacing, correct by one
-		const int xl = x0 + SPT - 1;
-		int i3 = (int) ((float) (xl - (la.sym[0] >> 2)) * ((float) dp.nicam_D / (float) dp.nicam_F));
-		i3 = max(0, min(la.nsym - 1, i3));
-		while(i3 + 1 < la.nsym && (la.sym[i3 + 1] >> 2) <= xl) i3++;
-		while(i3 > 0 && (la.sym[i3] >> 2) > xl) i3--;
-		const int sx3 = la.sym[i3] >> 2;
-		const int i2 = max(i3 - 1, 0);
-		const int r3 = la.symrow[i3], r2 = la.symrow[i2];
-		int bi[SPT], bq[SPT];
-		if((r3 | r2) >= 0)
-		{
-			// pulse-shaping table: one entry per sample and channel (htv_tables.c)
-			const int sx2 = la.sym[i2] >> 2;
-			#pragma unroll
-			for(int k = 0; k < SPT; k++)
-			{
-				const int x = x0 + k;
-				const bool cur = x >= sx3;
-				const int rows = cur ? r3 : r2;
-				const int phi = x - (cur ? sx3 : sx2);
-				bi[k] = __ldg(dt.nicam_lut + (rows & 0xFFFF) * dp.nicam_sps + phi);
-				bq[k] = __ldg(dt.nicam_lut + (rows >> 16) * dp.nicam_sps + phi);
-			}
-		}
-		else
-		{
-			// generic sum over the symbols whose pulse covers the samples (stream start, unusual rates)
-			#pragma unroll
-			for(int k = 0; k < SPT; k++) { bi[k] = 0; bq[k] = 0; }
-			for(int cnd = 0; cnd < NIC_CAND; cnd++)
-			{
-				const int i = i3 - cnd;
-				if(i < 0) break;
-				const int sy = la.sym[i];
-				const int d0 = x0 - (sy >> 2) + NIC_TPAD;           // the table is zero outside the pulse
-				if(d0 < 0) continue;
-				const int si = (sy & 1) ? 1 : -1, sq = (sy & 2) ? 1 : -1;
-				#pragma unroll
-				for(int k = 0; k < SPT; k++)
-				{
-					const int r = ntp[d0 + k];
-					bi[k] += r * si;
-					bq[k] += r * sq;
-				}
-			}
-		}
-		int ci = la.cc0 + x0;
-		while(ci >= dp.nicam_cc_len) ci -= dp.nicam_cc_len;
-		#pragma unroll
-		for(int k = 0; k < SPT; k++)
-		{
-			const htv_c16_t cc = dt.nicam_cc[ci];
-			if(++ci == dp.nicam_cc_len) ci = 0;
-			// the overlap-add ring holds at most 7 pulses of < 2^11: it never wraps an int16
-			oi[k] += (bi[k] * cc.i - bq[k] * cc.q) >> 15;
-			oq[k] += (bi[k] * cc.q + bq[k] * cc.i) >> 15;
-		}
-	}
-
-}
-
-// Mixers after the modulation (ref video.c:3466-3515), the channel combiner and the store.
+// Mixers after the modulation (htv_sound.cuh), the channel combiner and the store of 4 consecutive samples.
 // TY: the output has another sample type than int16 (dp.sample_type, htv_sample_type.h). The kernels that share this store
 // take it as a template argument, so that their int16 instantiations compile as if the conversion did not exist.
 template<bool TY>
-__device__ __forceinline__ void post_store(const htv_dparams_t &dp, const DevTables &dt, const LineAudio &la,
+__device__ __forceinline__ void mod_store(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
 	int x0, int row, int (&oi)[SPT], int (&oq)[SPT], int16_t *out, const int16_t *acc)
 {
 	const int W = dp.W;
-	// every addition above is an int16 wrap-around addition in the reference; wrapping once is the same
-	if(dp.swap_iq || dp.have_offset)
-	{
-		#pragma unroll
-		for(int k = 0; k < SPT; k++) { oi[k] = wrap16i(oi[k]); oq[k] = wrap16i(oq[k]); }
-	}
-
-	if(dp.swap_iq)
-	{
-		#pragma unroll
-		for(int k = 0; k < SPT; k++) { const int t = oi[k]; oi[k] = oq[k]; oq[k] = t; }
-	}
-
-	if(dp.have_offset)
-	{
-		for(int k = 0; k < SPT; k++)
-		{
-			const int x = x0 + k;
-			const int64_t m = la.m0 + x;
-			int bi, bq;
-			if(m < 32767)
-			{
-				const unsigned char st = dt.offset_start[m];
-				bi = -(st & 1); bq = -((st >> 1) & 1);
-			}
-			else
-			{
-				const int kk = (int) (m % 32767);
-				const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
-				const unsigned long long ph = la.off_phase0 + dp.offset_ang * (unsigned long long) (x + 1);
-				float sn, cs;
-				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
-				bi = min((int) floorf(amp * cs), 32767); bq = min((int) floorf(amp * sn), 32767);   // pi >> 16 <= 32767
-			}
-			const int ri = (oi[k] * bi - oq[k] * bq) >> 15, rq = (oi[k] * bq + oq[k] * bi) >> 15;
-			oi[k] = wrap16i(ri); oq[k] = wrap16i(rq);
-		}
-	}
+	kl_mix<-1, 1>(dp, dt, la, x0, oi, oq);
 
 	// ---- store (ref rf_file.c:97-116, 226-233 layout) ------------------------
 	// `acc` (same layout as `out`, may alias it): the stream to add this one into, int16 wrap per
@@ -1990,8 +1722,10 @@ __device__ __forceinline__ void post_store(const htv_dparams_t &dp, const DevTab
 	}
 }
 
+// Everything k_mod does for 4 consecutive samples once the composite window is in shared
+// memory. cwin[j] = composite sample x0 - 25 - CSKEW + j (16-byte aligned).
 template<int CSKEW, bool TY>
-__device__ __forceinline__ void mod_body(const htv_dparams_t &dp, const DevTables &dt, const LineAudio &la,
+__device__ __forceinline__ void mod_body(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
 	const int *cwin, const short *ntp, int x0, int row, int16_t *out, const int16_t *acc)
 {
 	const int W = dp.W;
@@ -2028,8 +1762,8 @@ __device__ __forceinline__ void mod_body(const htv_dparams_t &dp, const DevTable
 		for(int k = 0; k < SPT; k++) { oi[k] = cwin[k + HALO + CSKEW]; oq[k] = 0; }
 	}
 
-	sound_add<false>(dp, dt, la, ntp, x0, oi, oq);
-	post_store<TY>(dp, dt, la, x0, row, oi, oq, out, acc);
+	kl_sound<-1, 1>(dp, dt, la, ntp, x0, oi, oq);
+	mod_store<TY>(dp, dt, la, x0, row, oi, oq, out, acc);
 }
 
 
@@ -2071,7 +1805,7 @@ __device__ __forceinline__ unsigned long long block_sum_u64(unsigned long long v
 
 template<int NT>
 __global__ void __launch_bounds__(384)
-k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, int pre)
+k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2 *lap, const int16_t *comp, int pre)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = dp.W;
@@ -2079,14 +1813,14 @@ k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const L
 	const int CW = W4 + 2 * FOFF;
 	int *cw = reinterpret_cast<int *>(smem_raw);                    // index = x + FOFF
 	short *ntp = reinterpret_cast<short *>(cw + CW);
-	__shared__ LineAudio la;
+	__shared__ LineA2 la;
 	__shared__ unsigned long long red[12];
 	const int tid = threadIdx.x;
 
 	{
 		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
 		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineAudio) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
+		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
 	}
 	if(dp.have_nicam)
 	{
@@ -2135,7 +1869,7 @@ k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const L
 		}
 		#pragma unroll
 		for(int k = 0; k < SPT; k++) oq[k] = 0;
-		sound_add<true>(dp, dt, la, ntp, x0, oi, oq);                // only the I sum modulates (ref video.c:3460)
+		kl_sound<-1, 1, true>(dp, dt, &la, ntp, x0, oi, oq);         // only the I sum modulates (ref video.c:3460)
 		int16_t *b = dt.fmv_base + (size_t) blockIdx.x * W + x0;
 		#pragma unroll
 		for(int k = 0; k < SPT; k++)
@@ -2177,16 +1911,16 @@ __global__ void __launch_bounds__(1024) k_fmv_scan(const DevTables dt, int nrows
 
 template<bool TY>
 __global__ void __launch_bounds__(384)
-k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, int16_t *out,
+k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2 *lap, int16_t *out,
 	const int16_t *acc, int acc_rows, int out_row0)
 {
-	__shared__ LineAudio la;
+	__shared__ LineA2 la;
 	__shared__ unsigned long long wsum[12];
 	const int W = dp.W, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 	{
 		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
 		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineAudio) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
+		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
 	}
 	const int x0 = tid * SPT;
 	unsigned long long p[SPT];
@@ -2229,12 +1963,12 @@ k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		oi[k] = (min((int) floorf(amp * cs), 32767) * dp.fmv_level) >> 15;    // pi >> 16 <= 32767
 		oq[k] = (min((int) floorf(amp * sn), 32767) * dp.fmv_level) >> 15;
 	}
-	post_store<TY>(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
+	mod_store<TY>(dp, dt, &la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
 }
 
 template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
-k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int16_t *comp, int16_t *out,
+k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2 *lap, const int16_t *comp, int16_t *out,
 	const int16_t *acc, int acc_rows)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -2243,13 +1977,13 @@ k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAu
 	const int CW = W4 + 2 * EXT + 16;
 	int *cw = reinterpret_cast<int *>(smem_raw);                    // index = x + COFF
 	short *ntp = reinterpret_cast<short *>(cw + CW);                // padded NICAM pulse table
-	__shared__ LineAudio la;
+	__shared__ LineA2 la;
 	const int tid = threadIdx.x;
 
 	{
 		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
 		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineAudio) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
+		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
 	}
 	if(dp.have_nicam)
 	{
@@ -2285,12 +2019,12 @@ k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAu
 	const int x0 = tid * SPT;
 	if(x0 >= W) return;
 
-	mod_body<0, TY>(dp, dt, la, cw + x0 + COFF - HALO, ntp, x0, (int) blockIdx.x, out, (int) blockIdx.x < acc_rows ? acc : NULL);
+	mod_body<0, TY>(dp, dt, &la, cw + x0 + COFF - HALO, ntp, x0, (int) blockIdx.x, out, (int) blockIdx.x < acc_rows ? acc : NULL);
 }
 
 // ---------------------------------------------------------------------------
 // Persistent modulator: one CTA per SM slot loops over scan lines; the next line's composite
-// window (int32, written by k_raster) and its LineAudio descriptor are fetched by the TMA
+// window (int32, written by k_raster) and its LineA2 descriptor are fetched by the TMA
 // (cp.async.bulk global -> shared, mbarrier completion) into the other half of a double
 // buffer while the current line is computed, so no thread spends instructions on staging
 // and the load latency is hidden. Used whenever 4 | W (16-byte alignment of every window).
@@ -2321,22 +2055,19 @@ __device__ __forceinline__ void mbar_wait(void *bar, unsigned parity)
 
 template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
-k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const int *comp32, int nlines, int16_t *out,
+k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2 *lap, const int *comp32, int nlines, int16_t *out,
 	const int16_t *acc, int acc_rows)
 {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
 	const int W = dp.W;
 	const int NW = TWIN(W);
-	int *cwb[2];
-	LineAudio *lab[2];
-	cwb[0] = reinterpret_cast<int *>(smem_raw);
-	cwb[1] = cwb[0] + NW;
-	lab[0] = reinterpret_cast<LineAudio *>(cwb[1] + NW);
-	lab[1] = lab[0] + 1;
-	short *ntp = reinterpret_cast<short *>(lab[1] + 1);
+	// [buffer] composite windows, [buffer] descriptors, the NICAM pulse
+	int *cw0 = reinterpret_cast<int *>(smem_raw);
+	LineA2 *lab0 = reinterpret_cast<LineA2 *>(cw0 + 2 * NW);
+	short *ntp = reinterpret_cast<short *>(lab0 + 2);
 	__shared__ __align__(8) unsigned long long bar[2];
 	const int tid = threadIdx.x;
-	const unsigned bytes = (unsigned) (NW * sizeof(int) + sizeof(LineAudio));
+	const unsigned bytes = (unsigned) (NW * sizeof(int) + sizeof(LineA2));
 
 	if(dp.have_nicam)
 	{
@@ -2357,8 +2088,8 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	{
 		// the launch's composite stream starts one line early: line `row` begins at (row + 1) * W
 		asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(&bar[0])), "r"(bytes) : "memory");
-		tma_load(cwb[0], comp32 + ((size_t) row + 1) * W - TOFF, NW * sizeof(int), &bar[0]);
-		tma_load(lab[0], lap + row, sizeof(LineAudio), &bar[0]);
+		tma_load(cw0, comp32 + ((size_t) row + 1) * W - TOFF, NW * sizeof(int), &bar[0]);
+		tma_load(lab0, lap + row, sizeof(LineA2), &bar[0]);
 	}
 	unsigned phase[2] = { 0, 0 };
 	for(int it = 0; row < nlines; it++, row += gridDim.x)
@@ -2368,13 +2099,13 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		if(tid == 0 && nrow < nlines)
 		{
 			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(&bar[nb])), "r"(bytes) : "memory");
-			tma_load(cwb[nb], comp32 + ((size_t) nrow + 1) * W - TOFF, NW * sizeof(int), &bar[nb]);
-			tma_load(lab[nb], lap + nrow, sizeof(LineAudio), &bar[nb]);
+			tma_load(cw0 + nb * NW, comp32 + ((size_t) nrow + 1) * W - TOFF, NW * sizeof(int), &bar[nb]);
+			tma_load(lab0 + nb, lap + nrow, sizeof(LineA2), &bar[nb]);
 		}
 		mbar_wait(&bar[cb], phase[cb]);
 		phase[cb] ^= 1;
 		const int x0 = tid * SPT;
-		if(x0 < W) mod_body<3, TY>(dp, dt, *lab[cb], cwb[cb] + x0, ntp, x0, row, out, row < acc_rows ? acc : NULL);
+		if(x0 < W) mod_body<3, TY>(dp, dt, lab0 + cb, cw0 + cb * NW + x0, ntp, x0, row, out, row < acc_rows ? acc : NULL);
 		__syncthreads();                                            // everyone is done with this half before it is refilled
 	}
 }
@@ -2399,7 +2130,7 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 
 template<int MAXT, int MINB, bool TY = false>
 __global__ void __launch_bounds__(MAXT, MINB)
-k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineAudio *lap, const uint8_t *planes, size_t plane_stride,
+k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2 *lap, const uint8_t *planes, size_t plane_stride,
 	int pitch, int nlines, int16_t *out, const int16_t *acc, int acc_rows)
 {
 	extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -2411,11 +2142,11 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	unsigned char *pl0 = smem_raw;
 	uint4 *atab = reinterpret_cast<uint4 *>(pl0 + 4 * PB);              // [k-step][I hi, I lo, Q hi, Q lo][lane]
 	unsigned *fir0 = reinterpret_cast<unsigned *>(atab + MF_ATAB_WORDS / 4);
-	LineAudio *lab0 = reinterpret_cast<LineAudio *>(fir0 + 2 * FW);
+	LineA2 *lab0 = reinterpret_cast<LineA2 *>(fir0 + 2 * FW);
 	short *ntp = reinterpret_cast<short *>(lab0 + 3);
 	__shared__ __align__(8) unsigned long long bar[2];
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-	const unsigned bytes = (unsigned) (2 * WB + sizeof(LineAudio));
+	const unsigned bytes = (unsigned) (2 * WB + sizeof(LineA2));
 	const bool hasq = dp.vf_type == 3;
 
 	if(dp.have_nicam)
@@ -2448,7 +2179,7 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(&bar[0])), "r"(bytes) : "memory");
 		tma_load(pl0, src, WB, &bar[0]);
 		tma_load(pl0 + PB, src + plane_stride, WB, &bar[0]);
-		tma_load(lab0, lap + row, sizeof(LineAudio), &bar[0]);
+		tma_load(lab0, lap + row, sizeof(LineA2), &bar[0]);
 	}
 	unsigned phase[2] = { 0, 0 };
 	int l3 = 0;                                                         // it % 3: descriptor buffer of this line
@@ -2466,7 +2197,7 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 			asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(&bar[nb])), "r"(bytes) : "memory");
 			tma_load(pl0 + (2 * nb) * PB, src, WB, &bar[nb]);
 			tma_load(pl0 + (2 * nb + 1) * PB, src + plane_stride, WB, &bar[nb]);
-			tma_load(lab0 + n3, lap + nrow, sizeof(LineAudio), &bar[nb]);
+			tma_load(lab0 + n3, lap + nrow, sizeof(LineA2), &bar[nb]);
 		}
 		mbar_wait(&bar[cb], phase[cb]);
 		phase[cb] ^= 1;
@@ -2518,9 +2249,9 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 			oi[1] = (int) (short) (v.y & 0xFFFF); oq[1] = (int) v.y >> 16;
 			oi[2] = (int) (short) (v.z & 0xFFFF); oq[2] = (int) v.z >> 16;
 			oi[3] = (int) (short) (v.w & 0xFFFF); oq[3] = (int) v.w >> 16;
-			const LineAudio &la = lab0[l3];
-			sound_add<false>(dp, dt, la, ntp, x0, oi, oq);
-			post_store<TY>(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
+			const LineA2 *la = lab0 + l3;
+			kl_sound<-1, 1>(dp, dt, la, ntp, x0, oi, oq);
+			mod_store<TY>(dp, dt, la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
 		}
 		l3 = n3;
 	}
@@ -2579,21 +2310,21 @@ static const KSec ks_tab[] = {
 
 // the split modulators: k_mod (int16 stream), k_mod_tma (int32 stream, 4 | W), k_mod_mma (byte planes, video filter on);
 // an entry has the entry point of its own kernel only
-typedef void (*KModFn)(htv_dparams_t, DevTables, const LineAudio *, const int16_t *, int16_t *, const int16_t *, int);
-typedef void (*KModTmaFn)(htv_dparams_t, DevTables, const LineAudio *, const int *, int, int16_t *, const int16_t *, int);
-typedef void (*KModMmaFn)(htv_dparams_t, DevTables, const LineAudio *, const uint8_t *, size_t, int, int, int16_t *, const int16_t *, int);
+typedef void (*KModFn)(htv_dparams_t, DevTables, const LineA2 *, const int16_t *, int16_t *, const int16_t *, int);
+typedef void (*KModTmaFn)(htv_dparams_t, DevTables, const LineA2 *, const int *, int, int16_t *, const int16_t *, int);
+typedef void (*KModMmaFn)(htv_dparams_t, DevTables, const LineA2 *, const uint8_t *, size_t, int, int, int16_t *, const int16_t *, int);
 struct KMod { const char *name; KModFn mod; KModTmaFn tma; KModMmaFn mma; int maxt, minb, ty; };
 #define KM_ENTRY(T, B, TY) \
 	{ "k_mod", k_mod<T, B, TY>, NULL, NULL, T, B, TY }, { "k_mod_tma", NULL, k_mod_tma<T, B, TY>, NULL, T, B, TY }, \
 	{ "k_mod_mma", NULL, NULL, k_mod_mma<T, B, TY>, T, B, TY }
 static const KMod km_tab[] = { KM_ENTRY(256, 4, false), KM_ENTRY(256, 4, true), KM_ENTRY(384, 2, false), KM_ENTRY(384, 2, true) };
 
-typedef void (*KFmvBaseFn)(htv_dparams_t, DevTables, const LineAudio *, const int16_t *, int);
+typedef void (*KFmvBaseFn)(htv_dparams_t, DevTables, const LineA2 *, const int16_t *, int);
 struct KFmvBase { KFmvBaseFn fn; int nt; };
 #define KFB_ENTRY(NT) { k_fmv_base<NT>, NT }
 static const KFmvBase kfb_tab[] = { KFB_ENTRY(0), KFB_ENTRY(67), KFB_ENTRY(71) };
 
-typedef void (*KFmvModFn)(htv_dparams_t, DevTables, const LineAudio *, int16_t *, const int16_t *, int, int);
+typedef void (*KFmvModFn)(htv_dparams_t, DevTables, const LineA2 *, int16_t *, const int16_t *, int, int);
 struct KFmvMod { KFmvModFn fn; int ty; };
 #define KFM_ENTRY(TY) { k_fmv_mod<TY>, TY }
 static const KFmvMod kfm_tab[] = { KFM_ENTRY(false), KFM_ENTRY(true) };
@@ -2794,9 +2525,9 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 		{
 			p->plane_pitch = full ? 0 : mf_pitch(W);
 			p->mod_smem = (size_t) 4 * (p->plane_pitch ? mf_row_bytes(W) : mf_plane_bytes(W)) + sizeof(uint32_t) * MF_ATAB_WORDS +
-				sizeof(unsigned) * 2 * mf_tiles(W) * 4 * MF_ROWW + 3 * sizeof(LineAudio) + ntp + 128;
+				sizeof(unsigned) * 2 * mf_tiles(W) * 4 * MF_ROWW + 3 * sizeof(LineA2) + ntp + 128;
 		}
-		else if(tma) p->mod_smem = sizeof(int) * 2 * TWIN(W) + 2 * sizeof(LineAudio) + ntp + 128;
+		else if(tma) p->mod_smem = sizeof(int) * 2 * TWIN(W) + 2 * sizeof(LineA2) + ntp + 128;
 		else p->mod_smem = sizeof(int) * (W4 + 2 * EXT + 16) + ntp;
 		// --pixelrate: the raster runs in the pixel-rate context (PATH_RASTER), k_resample brings it to this one
 		if(p->path == PATH_SPLIT) p->raster = raster;
@@ -3089,7 +2820,7 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	// the side streams may still be ahead of the caller's; nothing of this encoder is freed under running work
 	cudaDeviceSynchronize();
 	for(int i = 0; i < d->nalloc; i++) cudaFree(d->alloc[i]);
-	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
 	if(d->h_map) cudaFreeHost(d->h_map);
 	if(d->h_ov_line) { cudaFreeHost(d->h_ov_line); cudaFreeHost(d->h_ov_meta); cudaFreeHost(d->h_ov_add); }
 	cudaFree(d->d_ov_line); cudaFree(d->d_ov_meta); cudaFree(d->d_ov_add);
@@ -3278,7 +3009,7 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	}
 	if(dp.have_nicam)
 	{
-		// its own stream beside the FM chain; `side` (where the descriptors follow) joins below
+		// its own stream beside the FM chain: the NICAM half of the sound descriptors follows it there
 		CK(cudaStreamWaitEvent(d->side2, d->ahead ? d->ev_up : d->ev_in, 0));
 		st = d->side2;
 		const int64_t s_lo = (int64_t) (((unsigned long long) (m0 > dp.nicam_ntaps ? m0 - dp.nicam_ntaps : 0) * dp.nicam_D) / dp.nicam_F);
@@ -3290,20 +3021,35 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 		k_nicam_scan<<<1, 1024, 0, st>>>(d->dt, k_lo, k_hi);
 		d->launches += 2;
 		d->nic_kc = k_hi;                                          // fstart[k_hi] is valid; recompute from there next time
-		if(d->plan.path != PATH_LINE && d->plan.path != PATH_SEC_LINE)
-		{
-			// the split kernels' descriptor kernel (on `side`) reads both chains
-			CK(cudaEventRecord(d->ev_nic, d->side2));
-			CK(cudaStreamWaitEvent(d->side, d->ev_nic, 0));
-		}
 	}
 	CK(cudaGetLastError());
 	return(HTV_OK);
 }
 
+// The sound descriptors of lines line0 .. line0 + n - 1 into la, on every path but the fused line kernel's (which runs
+// them ahead of the caller's stream): each half on the side stream of the pre-pass chain it depends on, behind this
+// call's place in the caller's stream st; ev_audio and ev_nic mark the two halves done
+static int launch_desc_a2(htv_dev_t *d, LineA2 *la, int64_t line0, int n, cudaStream_t st)
+{
+	if(!d->side_armed)
+	{
+		CK(cudaEventRecord(d->ev_in, st));
+		CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
+	}
+	CK(cudaStreamWaitEvent(d->side2, d->ev_in, 0));
+	const int dgrid = (n + KD_LINES * KD_WARPS - 1) / (KD_LINES * KD_WARPS);
+	k_line_desc_a2<1><<<dgrid, 32 * KD_WARPS, 0, d->side>>>(d->dp, d->dt, la, line0, n);
+	k_line_desc_a2<2><<<dgrid, 32 * KD_WARPS, 0, d->side2>>>(d->dp, d->dt, la, line0, n);
+	CK(cudaEventRecord(d->ev_audio, d->side));
+	CK(cudaEventRecord(d->ev_nic, d->side2));
+	d->side_armed = 0;
+	d->launches += 2;
+	return(HTV_OK);
+}
+
 // The plan's split modulator over n lines (htv_dev_render_lines, htv_dev_render_lines_rs): descriptors la, the composite
 // stream as k_raster / k_resample left it for this modulator (byte planes, int32, or the int16 `comp`), output o
-static void launch_mod(const htv_dev_t *d, int n, const LineAudio *la, const int16_t *comp, int16_t *o, const int16_t *acc,
+static void launch_mod(const htv_dev_t *d, int n, const LineA2 *la, const int16_t *comp, int16_t *o, const int16_t *acc,
 	int acc_rows, cudaStream_t st)
 {
 	const DevPlan &p = d->plan;
@@ -3329,17 +3075,16 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		cudaStreamSynchronize(d->side);
 		cudaStreamSynchronize(d->side2);
 		cudaStreamSynchronize(d->side3);
-		cudaFree(d->d_desc_r); cudaFree(d->d_desc_a); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
-		d->d_desc_r = d->d_desc_a = d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
+		cudaFree(d->d_desc_r); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
+		d->d_desc_r = d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
 		d->desc_cap = 0;
 		if(p.path == PATH_LINE) CK(cudaMalloc(&d->d_desc_r2, 2 * sizeof(LineR2) * ((size_t) nlines + 2)));
 		else CK(cudaMalloc(&d->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 3)));
-		if(p.path == PATH_LINE || p.path == PATH_SEC_LINE) CK(cudaMalloc(&d->d_desc_a2, 2 * sizeof(LineA2) * ((size_t) nlines + 1)));
+		CK(cudaMalloc(&d->d_desc_a2, (p.path == PATH_LINE ? 2 : 1) * sizeof(LineA2) * ((size_t) nlines + 1)));
 		if(p.ks) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) nlines + 3)));
-		else CK(cudaMalloc(&d->d_desc_a, sizeof(LineAudio) * ((size_t) nlines + 1)));
 		d->desc_cap = nlines;
 	}
-	LineDescs ld = { (LineRaster *) d->d_desc_r + 1, (LineAudio *) d->d_desc_a };
+	LineRaster *lr0 = (LineRaster *) d->d_desc_r + 1;
 	if(p.path == PATH_LINE)
 	{
 		// one persistent launch for the whole call: every CTA walks its own run of consecutive lines
@@ -3394,27 +3139,11 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		CK(cudaGetLastError());
 		return(HTV_OK);
 	}
-	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, ld, line0, nlines, p.ks ? (LineS2 *) d->d_desc_s2 : NULL);
-	if(!d->side_armed)
-	{
-		CK(cudaEventRecord(d->ev_in, st));
-		CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
-	}
+	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, lr0, line0, nlines, p.ks ? (LineS2 *) d->d_desc_s2 : NULL);
+	d->launches++;
+	// la2[i] <-> line line0 - fm_skip + i
 	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
-	if(p.path == PATH_SEC_LINE)
-	{
-		// the sound descriptors of the fused line kernel, each half on the side stream of the pre-pass chain it depends on
-		const int dgrid = (nlines + KD_LINES * KD_WARPS - 1) / (KD_LINES * KD_WARPS);
-		CK(cudaStreamWaitEvent(d->side2, d->ev_in, 0));
-		k_line_desc_a2<1><<<dgrid, 32 * KD_WARPS, 0, d->side>>>(d->dp, d->dt, la2, line0, nlines);
-		k_line_desc_a2<2><<<dgrid, 32 * KD_WARPS, 0, d->side2>>>(d->dp, d->dt, la2, line0, nlines);
-		CK(cudaEventRecord(d->ev_nic, d->side2));
-		d->launches++;
-	}
-	else k_line_desc_a<<<(nlines + fm_skip + 63) / 64, 64, 0, d->side>>>(d->dp, d->dt, ld, line0 - fm_skip, nlines + fm_skip);
-	CK(cudaEventRecord(d->ev_audio, d->side));
-	d->launches += 2;
-	d->side_armed = 0;
+	if(launch_desc_a2(d, la2, line0 - fm_skip, nlines + fm_skip, st) != HTV_OK) return(HTV_ERROR);
 	bool joined = false;
 	for(int done = 0; done < nlines; done += d->sub_lines)
 	{
@@ -3428,7 +3157,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		if(d->dp.colour_mode == HTV_SECAM)
 		{
 			// rows 0 .. n+2 <-> lines first-2 .. first+n; the chain covers rows 0 .. n+1
-			const LineRaster *lr = ld.r + done - 1;
+			const LineRaster *lr = lr0 + done - 1;
 			if(p.ks)
 			{
 				// rows 0 .. n+2: their own compact descriptors, then runs of rows per persistent CTA
@@ -3514,20 +3243,20 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		else
 		{
 			// raster lines done-1 .. done+n (descriptor index = line - (line0 - 1))
-			k_raster<<<n + 2, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, ld.r + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, p.plane_pitch);
+			k_raster<<<n + 2, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, lr0 + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, p.plane_pitch);
 			d->launches++;
 		}
 		if(!joined)
 		{
 			CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
-			if(p.path == PATH_SEC_LINE) CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
+			CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
 			joined = true;
 		}
 		if(d->timing && last) cudaEventRecord(d->ev0, st);
 		if(p.path == PATH_FMV)
 		{
 			const int pre = fm_skip && done == 0 ? 1 : 0, rows = n + pre;
-			const LineAudio *lap = ld.a + done + fm_skip - pre;
+			const LineA2 *lap = la2 + done + fm_skip - pre;
 			p.fmv_base->fn<<<rows, p.line_threads, p.fmv_smem, st>>>(d->dp, d->dt, lap, cstream, pre);
 			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, rows);
 			p.fmv_mod->fn<<<rows, p.line_threads, 0, st>>>(d->dp, d->dt, lap, o, acc, acc_rows, -pre);
@@ -3541,7 +3270,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 			const int grid = (n + run - 1) / run;
 			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(d->dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp);
 		}
-		else launch_mod(d, n, ld.a + done, cstream, o, acc, acc_rows, st);
+		else launch_mod(d, n, la2 + done, cstream, o, acc, acc_rows, st);
 		strcpy(d->kname, p.kname);
 		d->launches++;
 		if(last) d->last_mod_lines = n;
@@ -3606,38 +3335,30 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	{
 		cudaStreamSynchronize(st);
 		cudaStreamSynchronize(d->side);
-		cudaFree(d->d_desc_r); cudaFree(d->d_desc_a);
-		d->d_desc_r = d->d_desc_a = NULL;
+		cudaStreamSynchronize(d->side2);
+		cudaFree(d->d_desc_a2);
+		d->d_desc_a2 = NULL;
 		d->desc_cap = 0;
-		CK(cudaMalloc(&d->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 3)));
-		CK(cudaMalloc(&d->d_desc_a, sizeof(LineAudio) * ((size_t) nlines + 1)));
+		CK(cudaMalloc(&d->d_desc_a2, sizeof(LineA2) * ((size_t) nlines + 1)));
 		d->desc_cap = nlines;
 	}
 	if(nlines + 1 > r->desc_cap)
 	{
 		cudaStreamSynchronize(st);
-		cudaFree(r->d_desc_r); cudaFree(r->d_desc_a);
-		r->d_desc_r = r->d_desc_a = NULL;
+		cudaFree(r->d_desc_r);
+		r->d_desc_r = NULL;
 		r->desc_cap = 0;
 		CK(cudaMalloc(&r->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 4)));
-		CK(cudaMalloc(&r->d_desc_a, sizeof(LineAudio) * ((size_t) nlines + 2)));
 		r->desc_cap = nlines + 1;
 	}
 	// raster descriptors for lines line0 - 2 .. line0 + nlines + 1 (one line more than without a resampler:
 	// the emitted line t is resampled line t + 1 and the video filter looks into t + 2)
-	LineDescs ldr = { (LineRaster *) r->d_desc_r + 1, (LineAudio *) r->d_desc_a };
-	LineDescs lda = { (LineRaster *) d->d_desc_r + 1, (LineAudio *) d->d_desc_a };
-	k_line_desc_r<<<(nlines + 4 + 63) / 64, 64, 0, st>>>(r->dp, r->dt, ldr, line0, nlines + 1, NULL);
-	if(!d->side_armed)
-	{
-		CK(cudaEventRecord(d->ev_in, st));
-		CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
-	}
-	k_line_desc_a<<<(nlines + 63) / 64, 64, 0, d->side>>>(d->dp, d->dt, lda, line0, nlines);
-	CK(cudaEventRecord(d->ev_audio, d->side));
-	d->side_armed = 0;
+	LineRaster *lr0 = (LineRaster *) r->d_desc_r + 1;
+	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
+	k_line_desc_r<<<(nlines + 4 + 63) / 64, 64, 0, st>>>(r->dp, r->dt, lr0, line0, nlines + 1, NULL);
+	d->launches++;
+	if(launch_desc_a2(d, la2, line0, nlines, st) != HTV_OK) return(HTV_ERROR);
 	bool joined = false;
-	d->launches += 2;
 	const int Ws = d->dp.W, Wp = r->dp.W;
 	int sub = d->sub_lines < r->sub_lines ? d->sub_lines : r->sub_lines;
 	for(int done = 0; done < nlines; done += sub)
@@ -3648,14 +3369,19 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * Ws * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
 		// raster lines line0 + done - 1 .. line0 + done + n + 1 -> rows 0 .. n + 2 of the raster context's int16 stream
-		k_raster<<<n + 3, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt, ldr.r + done, r->d_comp, NULL, NULL, 0, 0);
+		k_raster<<<n + 3, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt, lr0 + done, r->d_comp, NULL, NULL, 0, 0);
 		// resampled lines line0 + done .. line0 + done + n + 1 -> rows 0 .. n + 1 of this context's scratch
 		k_resample<<<n + 2, p.line_threads, 0, st>>>(r->d_comp, Wp, Ws, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
 			d->d_planes, d->plane_stride, d->d_comp32, d->d_comp);
 		d->launches += 2;
-		if(!joined) { CK(cudaStreamWaitEvent(st, d->ev_audio, 0)); joined = true; }
+		if(!joined)
+		{
+			CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
+			CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
+			joined = true;
+		}
 		if(d->timing && last) cudaEventRecord(d->ev0, st);
-		launch_mod(d, n, lda.a + done, d->d_comp, o, acc, acc_rows, st);
+		launch_mod(d, n, la2 + done, d->d_comp, o, acc, acc_rows, st);
 		d->launches++;
 		strcpy(d->kname, p.kname);
 		if(last) d->last_mod_lines = n;

@@ -15,21 +15,18 @@
 // samples in the layout the m16n8k32 accumulators have anyway: lane = 4g + t holds x = 128 tile + 32 t + g + 8 j,
 // j = 0..3 (htv_mma_fir.h: mf_out_x). Both filters leave their results in exactly the registers the next
 // stage needs - no exchange through shared memory, and all four samples of a lane fall into one 32-sample
-// block, which is what the per-line sound descriptors are indexed by. Loads and stores with a stride of 8
-// samples between a lane's values are still sector-exact (8 lanes x 4 bytes = one 32-byte sector).
+// block, which is what the per-line sound descriptors are indexed by: the sound carriers and mixers are htv_sound.cuh's
+// with S = 8. Loads and stores with a stride of 8 samples between a lane's values are still sector-exact (8 lanes x 4
+// bytes = one 32-byte sector).
 
 #define KL_LEAD   MF_LEAD   // composite row: byte i = sample i - 32 of the line (htv_mma_fir.h pitched row)
 #define KL_UVLEAD MF_LP_LEAD // chroma planes: byte i = sample i - 8
-#define KL_BIAS   2048      // NICAM pulse-table index bias (LineAudio.symb)
 
 __device__ __forceinline__ int kl_row_bytes(int W) { return(mf_row_bytes(W) + 16); }
 __device__ __forceinline__ int kl_uv_bytes(int W) { return(MF_TILE * mf_tiles(W) + 32); }
 
 // tap operand of the chroma low-pass (one k-step of 32): mf_lp_a_word (htv_mma_fir.h, shared with the host-side emulation)
 #define kl_chroma_a_word mf_lp_a_word
-
-// one complex int16 table entry through the read-only path: x = i, y = q
-__device__ __forceinline__ short2 kl_ldc16(const htv_c16_t *p) { return(__ldg(reinterpret_cast<const short2 *>(p))); }
 
 // the three partial sums of a byte-split contraction back to the reference's int32 accumulator (mf_combine:
 // 65536 hh + 256 mid + ll with wrap-around), as two shift-adds, then >> 15
@@ -40,168 +37,7 @@ __device__ __forceinline__ int kl_acc15(int hh, int mid, int ll)
 }
 __device__ __forceinline__ int kl_fir_out(int hh, int mid, int ll) { return(sat16i(kl_acc15(hh, mid, ll))); }
 
-// SND: the sound carriers and post-modulation stages an instantiation has compiled in, as a mask of the flags below, or
-// -1 for the general form, which tests dp on every line. They are fixed for an encoder's life, so the host picks the
-// instantiation from dp (kl_snd_mask). Only the mask of the PAL systems with FM mono and NICAM on a VSB carrier has its
-// own instantiation, and only at W = 1024 (16 Msps), with the width compiled in too (WC); at 320 threads the fixed form
-// spills.
-#define KL_FM   1
-#define KL_AM   2
-#define KL_NIC  4
-#define KL_OFF  8
-#define KL_SWAP 16
-#define KL_CPX  32
-#define KL_SND_FM_NICAM (KL_FM | KL_NIC | KL_CPX)
-#define KL_HAS(SND, BIT, RT) ((SND) < 0 ? (RT) != 0 : ((SND) & (BIT)) != 0)
-
-static inline int kl_snd_mask(const htv_dparams_t &dp)
-{
-	return((dp.have_fm ? KL_FM : 0) | (dp.have_am ? KL_AM : 0) | (dp.have_nicam ? KL_NIC : 0) |
-		(dp.have_offset ? KL_OFF : 0) | (dp.swap_iq ? KL_SWAP : 0) | (dp.complex_out ? KL_CPX : 0));
-}
-
-// ---- sound carriers for the four samples of a lane (strided by 8) --------------------------------------------
-// Same arithmetic as sound_add<false> (ref video.c:3261-3450, nicam728.c:342-411); what differs is how a lane
-// finds its audio segment and NICAM symbol: all four samples lie in the 32-sample block b = xb >> 5, for which
-// the line descriptor (in shared memory) lists the segment / symbol in effect at the block's first sample, and
-// at most one boundary of either kind falls inside a block.
-// FM carrier: one sin/cos for the lane's first sample, the other three by rotating with the segment's
-// (cos, sin) of 8 angle steps - unless an audio-segment boundary or a renormalisation of the reference's
-// phasor (every 32 767 samples) falls between the lane's samples; then every sample gets its own.
-template<int SND>
-__device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
-	const short *ntp, int xb, int (&oi)[4], int (&oq)[4])
-{
-	const int b = xb >> 5;
-	const bool fm = KL_HAS(SND, KL_FM, dp.have_fm), am = KL_HAS(SND, KL_AM, dp.have_am);
-	if(fm || am)
-	{
-		const int sg = la->fm_blk[b];
-		const int nb = la->seg_x[sg + 1];
-		const int sg1 = min(sg + 1, MAX_SEGS - 1);
-		int kk = la->kk0 + xb;
-		if(kk >= 32767) kk -= 32767;
-		// amplitude of the reference's Q31 phasor kk + 1 multiplications after a renormalisation
-		const float kf = (float) (kk + 1);
-		const bool mixed = (nb > xb && nb <= xb + 24) || kk + 25 > 32767;
-		if(fm)
-		{
-			if(!mixed)
-			{
-				const int s0 = xb >= nb ? sg1 : sg;
-				const unsigned long long ph = la->seg_phase[s0] + la->seg_ang[s0] * (unsigned long long) xb;
-				const float2 rot = la->seg_rot[s0];
-				float sn, cs;
-				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);   // pi / 2^31
-				float amp = 32767.99998f - kf * 1.52587890625e-5f;
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					oi[j] += (__float2int_rd(amp * cs) * dp.fm_level) >> 15;
-					oq[j] += (__float2int_rd(amp * sn) * dp.fm_level) >> 15;
-					const float c2 = __fmaf_rn(cs, rot.x, -(sn * rot.y)), s2 = __fmaf_rn(sn, rot.x, cs * rot.y);
-					cs = c2; sn = s2;
-					amp -= 8.0f * 1.52587890625e-5f;
-				}
-			}
-			else
-			{
-				const unsigned long long angA = la->seg_ang[sg], angB = la->seg_ang[sg1];
-				unsigned long long phA = la->seg_phase[sg] + angA * (unsigned long long) xb;
-				unsigned long long phB = la->seg_phase[sg1] + angB * (unsigned long long) xb;
-				const unsigned long long stA = angA << 3, stB = angB << 3;
-				float kq = kf;
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					const unsigned long long ph = xb + 8 * j >= nb ? phB : phA;
-					if(kq > 32767.0f) kq -= 32767.0f;
-					const float amp = 32767.99998f - kq * 1.52587890625e-5f;
-					float sn, cs;
-					__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
-					oi[j] += (__float2int_rd(amp * cs) * dp.fm_level) >> 15;
-					oq[j] += (__float2int_rd(amp * sn) * dp.fm_level) >> 15;
-					phA += stA; phB += stB; kq += 8.0f;
-				}
-			}
-		}
-		if(am)
-		{
-			unsigned long long phM = la->am_phase0 + dp.am_ang * (unsigned long long) (xb + 1);
-			const unsigned long long stM = dp.am_ang << 3;
-			const int amA = (la->seg_am[sg] + 32768) / 2, amB = (la->seg_am[sg1] + 32768) / 2;
-			float kq = kf;
-			#pragma unroll
-			for(int j = 0; j < 4; j++)
-			{
-				if(kq > 32767.0f) kq -= 32767.0f;
-				const float amp = 32767.99998f - kq * 1.52587890625e-5f;
-				float sn, cs;
-				__sincosf((float) (int) (phM >> 32) * 1.4629180792671596e-9f, &sn, &cs);
-				const int smp = xb + 8 * j >= nb ? amB : amA;
-				oi[j] += (((__float2int_rd(amp * cs) * smp) >> 15) * dp.am_level) >> 15;
-				oq[j] += (((__float2int_rd(amp * sn) * smp) >> 15) * dp.am_level) >> 15;
-				phM += stM; kq += 8.0f;
-			}
-		}
-	}
-
-	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
-	{
-		int bi[4], bq[4];
-		if(!la->nic_generic)
-		{
-			// pulse-shaping table (htv_tables.c): one entry per sample and channel, index = base + x
-			const int ib = la->nic_blk[b];
-			const uint2 cur = la->symb[ib], nxt = la->symb[ib + 1];
-			const int nb = (int) nxt.y;
-			const int16_t *lut = dt.nicam_lut - KL_BIAS + xb;
-			#pragma unroll
-			for(int j = 0; j < 4; j++)
-			{
-				const unsigned w = xb + 8 * j >= nb ? nxt.x : cur.x;
-				bi[j] = __ldg(lut + 8 * j + (w & 0xFFFFu));
-				bq[j] = __ldg(lut + 8 * j + (w >> 16));
-			}
-		}
-		else
-		{
-			// generic sum over the symbols whose pulse covers the sample (stream start, unusual rates)
-			#pragma unroll
-			for(int j = 0; j < 4; j++)
-			{
-				const int x = xb + 8 * j;
-				int i3 = 0;
-				const int ns = la->nsym;
-				while(i3 + 1 < ns && (int) la->symb[i3 + 1].y <= x) i3++;
-				bi[j] = 0; bq[j] = 0;
-				for(int cnd = 0; cnd < NIC_CAND; cnd++)
-				{
-					const int i = i3 - cnd;
-					if(i < 0) break;
-					const int sy = la->symc[i];
-					const int d0 = x - (int) la->symb[i].y + NIC_TPAD;      // the table is zero outside the pulse
-					if(d0 < 0) continue;
-					const int r = ntp[d0];
-					bi[j] += (sy & 1) ? r : -r;
-					bq[j] += (sy & 2) ? r : -r;
-				}
-			}
-		}
-		// carrier table extended past its period (htv_tables.c): cc0 + x never wraps
-		const htv_c16_t *ccp = dt.nicam_cc + la->cc0 + xb;
-		#pragma unroll
-		for(int j = 0; j < 4; j++)
-		{
-			const short2 cc = kl_ldc16(ccp + 8 * j);
-			// the overlap-add ring holds at most 7 pulses of < 2^11: it never wraps an int16
-			oi[j] += (bi[j] * cc.x - bq[j] * cc.y) >> 15;
-			oq[j] += (bi[j] * cc.y + bq[j] * cc.x) >> 15;
-		}
-	}
-}
-
-// Mixers after the modulation (ref video.c:3466-3515), channel combiner, store - post_store for the strided layout.
+// Mixers after the modulation (htv_sound.cuh), channel combiner, store in the strided layout.
 // ST: the sample type the store converts to (htv_sample_type.h), -1 for dp.sample_type at run time. The channel combiner
 // (`acc`, int16 in the output layout) still adds in int16 with wrap-around; the conversion is the last step, as the
 // reference's file sink converts what the video stage handed it. A lane stores each of its samples on its own (1, 2,
@@ -210,40 +46,7 @@ template<bool FULL, int SND, int ST>
 __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
 	int W, int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
 {
-	if(KL_HAS(SND, KL_SWAP, dp.swap_iq))
-	{
-		#pragma unroll
-		for(int j = 0; j < 4; j++) { const int t = oi[j]; oi[j] = oq[j]; oq[j] = t; }
-	}
-	if(KL_HAS(SND, KL_OFF, dp.have_offset))
-	{
-		const long long m0 = la->m0;
-		const unsigned long long off0 = la->off_phase0;
-		#pragma unroll
-		for(int j = 0; j < 4; j++)
-		{
-			const int x = xb + 8 * j;
-			const long long m = m0 + x;
-			const int vi = wrap16i(oi[j]), vq = wrap16i(oq[j]);
-			int bi, bq;
-			if(m < 32767)
-			{
-				const unsigned char st = dt.offset_start[m];
-				bi = -(st & 1); bq = -((st >> 1) & 1);
-			}
-			else
-			{
-				const int kk = (int) (m % 32767);
-				const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
-				const unsigned long long ph = off0 + dp.offset_ang * (unsigned long long) (x + 1);
-				float sn, cs;
-				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
-				bi = min(__float2int_rd(amp * cs), 32767); bq = min(__float2int_rd(amp * sn), 32767);   // pi >> 16 <= 32767
-			}
-			oi[j] = (vi * bi - vq * bq) >> 15;
-			oq[j] = (vi * bq + vq * bi) >> 15;
-		}
-	}
+	kl_mix<SND, 8>(dp, dt, la, xb, oi, oq);
 	const size_t lbase = (size_t) row * (size_t) W;
 	if constexpr(ST != HTV_TYPE_INT16)
 	{
@@ -584,7 +387,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		if(FULL || xb < W)
 		{
 			const LineA2 *la = sla + (mrow & 1);
-			kl_sound<SND>(dp, dt, la, ntp, xb, oi, oq);
+			kl_sound<SND, 8>(dp, dt, la, ntp, xb, oi, oq);
 			kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
 		}
 	}

@@ -1,7 +1,7 @@
 /* hacktv_b200 - the file sink's sample types (ref rf_file.c: the twelve _rf_file_write_* writers, rf.h:31-36).
  *
  * The one definition of how an int16 output value becomes a uint8, int8, uint16, int16, int32 or float sample.
- * The line kernels' stores (kl_post_store in htv_line.cuh, post_store in htv_kernels.cu), htv_convert's kernel,
+ * The line kernels' stores (kl_post_store in htv_line.cuh, mod_store in htv_kernels.cu), htv_convert's kernel,
  * the host layer (sizes) and the CPU check tests/sample_type_emu.c all include this header.
  *
  * x is always an int16 value (already wrapped): the reference converts what the video stage handed to rf_write.
