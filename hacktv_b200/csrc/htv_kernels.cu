@@ -59,7 +59,6 @@ struct DevTables {
 	const int16_t *tmpl_out, *tmpl_keep;   // line templates: blank + sync pulses (htv_tables.c build_templates)
 	const uint8_t *tmpl_keep_any;
 	const uint16_t *codes;
-	const int16_t *pulse_values;
 	const double *glut;
 	const short4 *yuv_lut;            // [2^24] RGB -> (y, u, v, 0), the reference's yuv_level_lookup (video.c:3905-3960)
 	const htv_c16_t *clut;
@@ -215,11 +214,10 @@ struct htv_dev_t {
 	int r2_armed;
 	int side_armed;
 	int ev_pending;
-	void *d_desc_r;                   // LineRaster[cap + 2]
-	void *d_desc_r2;                  // LineR2[cap + 2] x 2 (fused line kernel)
+	void *d_desc_r2;                  // LineR2[cap + 2] (x 2 for the fused line kernel): the raster of PAL / NTSC / mono
 	void *d_desc_a2;                  // LineA2[cap + 1] (x 2 for the fused line kernel)
-	void *d_desc_s2;                  // LineS2[cap + 3] (SECAM raster in the fused kernel's form)
-	int desc_cap;
+	void *d_desc_s2;                  // LineS2[cap + 3]: the raster of SECAM
+	int desc_cap;                     // lines per call the descriptor buffers hold (desc_reserve)
 	int kl_ctas;                      // persistent CTAs of the fused kernels (k_line, k_sec_raster)
 	char kname[192];                  // the line kernel(s) the last render launched, with their template arguments (htv_line_kernel)
 	SecScratch sec;                   // SECAM scratch (same sub-batch rows as d_comp)
@@ -602,35 +600,9 @@ __global__ void __launch_bounds__(1024) k_nicam_scan(const DevTables dt, int64_t
 #define UOFF (EXT + 8)                // chroma window index = x + UOFF
 #define NIC_CAND 7                    // NICAM symbols that can overlap 4 consecutive samples
 #define NIC_TPAD 8                    // zero entries in front of the padded NICAM pulse table
-#define MAX_ENT 6                     // sync pulse pieces that can land on one line (2 previous + 2 own + 2 next)
 #define MAX_SEGS 6                    // audio samples overlapping one scan line (+1)
 #define MAX_SYMS 48                   // NICAM symbols overlapping one scan line
 #define MAX_BLKS 48                   // 32-sample blocks of a line (W <= 1536)
-
-// What the raster needs to know about a line (also read for the two neighbours)
-struct __align__(16) LineRaster {
-	int valid;                        // 0: before the stream (the filter window starts zeroed)
-	int frame, line, code;            // 1-based, as the reference counts
-	int pal;                          // 0 no chroma, +1 / -1 V-switch
-	int al, ar;                       // active sample range [al, ar), -1 if none
-	unsigned int clut_off;
-	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
-	int nent, pad0;
-	int ent_base[MAX_ENT], ent_len[MAX_ENT], ent_pos[MAX_ENT], ent_keep[MAX_ENT];
-	// SECAM (ref video.c:3068-3233)
-	int sec_proc;                     // the line carries a chroma subcarrier
-	int sec_dr;                       // 1: D'r line (uses v), 0: D'b (uses u)
-	int sec_sign;                     // subcarrier phase reset: +1 / -1
-	int sec_sr;                       // end of the modulated range (start is burst_left)
-	int sec_clear;                    // the line-average store is cleared at this line (line 1 / hline)
-	int sec_prev_kind;                // what the store holds: 0 zeros, 1 black, 2 a picture row
-	int sec_prev_comp;                // ... and which component of it: 1 u, 2 v
-	int pad1;
-	long long sec_prev_row;           // pixel offset of that row
-	// VBI overlay on this line (ref vbidata.c:186-239, wss.c:182-185): I[from, to) = value, then I += add
-	int ov_from, ov_to, ov_value, ov_add; // ov_add: row of dt.ov_add, -1 none; ov_from >= ov_to: no replace
-	int ov_any, pad2;
-};
 
 // Sound-carrier state of a line for the sound stage (htv_sound.cuh), built by k_line_desc_a2 (one warp per line)
 struct __align__(16) LineA2 {
@@ -651,22 +623,43 @@ struct __align__(16) LineA2 {
 	int pad[2];
 };
 
-// What the raster half needs to know about a line (64 bytes, read through the read-only path)
+// Raster descriptors: what the raster kernels need to know about a scan line, one form per colour system (64 bytes
+// each, read as four int4). Blanking and sync come from the line templates (htv_tables.c build_templates): row `tmpl`
+// of dt.tmpl_out outside the picture [al, ar), the picture value plus row `tmpl` of dt.tmpl_keep inside it.
+// PAL / NTSC / mono (k_line, k_raster)
 struct __align__(16) LineR2 {
 	int valid;                        // 0: before the stream
 	int tmpl;                         // row of the line templates
 	int al, ar;                       // active sample range [al, ar), -1 if none
 	int pal;                          // 0 no chroma, +1 / -1 V-switch
 	int keep;                         // the template's keep part is non-zero somewhere
+	// VBI overlay on this line (ref vbidata.c:186-239, wss.c:182-185): I[from, to) = value, then I += add
 	int ov_any, ov_from;
 	unsigned int clut_off;
-	int ov_to, ov_value, ov_add;
+	int ov_to, ov_value, ov_add;      // ov_add: row of dt.ov_add, -1 none; ov_from >= ov_to: no replace
 	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
 	long long pad;
 };
 static_assert(sizeof(LineR2) == 64, "LineR2 is read as four int4");
 
-static_assert(sizeof(LineRaster) % 16 == 0 && sizeof(LineA2) % 16 == 0, "descriptors are copied as int4");
+// SECAM (k_sec_raster, k_raster_secam and the chrominance chain, ref video.c:3068-3233)
+struct __align__(16) LineS2 {
+	int valid;                        // 0: before the stream
+	int tmpl;                         // row of the line templates
+	int al, ar;                       // active sample range [al, ar), -1 if none
+	int keep;                         // the template's keep part is non-zero somewhere
+	int sec_proc, sec_dr;             // the line carries a subcarrier; 1: D'r line (uses v), 0: D'b (uses u)
+	int sec_prev_kind;                // what the line-average store holds: 0 zeros, 1 black, 2 a picture row
+	int sec_prev_comp;                // ... and which component of it: 1 u, 2 v
+	int sec_sign;                     // subcarrier phase reset: +1 / -1
+	int sec_sr;                       // end of the modulated range (start is burst_left)
+	int sec_clear;                    // the line-average store is cleared at this line (line 1 / hline)
+	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
+	long long sec_prev_row;           // pixel offset of the stored row
+};
+static_assert(sizeof(LineS2) == 64, "LineS2 is read as four int4");
+
+static_assert(sizeof(LineA2) % 16 == 0, "descriptors are copied as int4");
 
 // frame / line / picture row of scan line L; L < 0 are the pipeline-fill lines the reference's
 // SECAM stage sees before line 1 (frame 1, line 0: an all-black active line, ref video.c:4665-4667)
@@ -679,6 +672,7 @@ __device__ __forceinline__ void line_numbers(const htv_dparams_t &dp, const DevT
 	frame = (int) (f0 + 1);
 	line = (int) (L - f0 * dp.lines) + 1;
 	code = dt.codes[line];
+	// source row (ref video.c:2812-2895): a progressive source on an interlaced raster shifts down one row
 	int vy;
 	if(dp.raster == HTV_RASTER_625) vy = line < 313 ? (line - 23) * 2 : (line - 336) * 2 + 1;
 	else vy = line < 265 ? (line - 23) * 2 : (line - 286) * 2 + 1;
@@ -695,16 +689,15 @@ __device__ __forceinline__ void line_numbers(const htv_dparams_t &dp, const DevT
 	}
 }
 
-__device__ void line_secam(const htv_dparams_t &dp, const DevTables &dt, int64_t L, LineRaster &li)
+// the SECAM fields of line L, whose frame / line / code line_numbers gave
+__device__ void line_secam(const htv_dparams_t &dp, const DevTables &dt, int64_t L, int frame, int line, int code, LineS2 &o)
 {
-	int frame, line, code; long long row;
-	line_numbers(dp, dt, L, frame, line, code, row);
-	li.sec_proc = (code & (HTV_LC_LEFT_ACTIVE | HTV_LC_RIGHT_ACTIVE)) != 0;
-	li.sec_dr = ((frame * dp.lines) + line) & 1;
-	li.sec_sign = ((frame * dp.lines) + line) % 3 == 0 ? 1 : -1;
-	li.sec_sr = (code & HTV_LC_RIGHT_ACTIVE) ? dp.burst_left + dp.burst_width : dp.half_width;
-	li.sec_clear = L >= 0 && (line == 1 || line == dp.hline);
-	li.sec_prev_kind = 0; li.sec_prev_comp = 1; li.sec_prev_row = -1;
+	o.sec_proc = (code & (HTV_LC_LEFT_ACTIVE | HTV_LC_RIGHT_ACTIVE)) != 0;
+	o.sec_dr = ((frame * dp.lines) + line) & 1;
+	o.sec_sign = ((frame * dp.lines) + line) % 3 == 0 ? 1 : -1;
+	o.sec_sr = (code & HTV_LC_RIGHT_ACTIVE) ? dp.burst_left + dp.burst_width : dp.half_width;
+	o.sec_clear = L >= 0 && (line == 1 || line == dp.hline);
+	o.sec_prev_kind = 0; o.sec_prev_comp = 1; o.sec_prev_row = -1;
 	// what the vertical-average store holds when this line reads it (ref video.c:3149-3196):
 	// the other component of the last processed line, unless a clearing line came in between
 	for(int64_t M = L; M >= L - dp.lines; M--)
@@ -716,86 +709,68 @@ __device__ void line_secam(const htv_dparams_t &dp, const DevTables &dt, int64_t
 		line_numbers(dp, dt, M - 1, f2, l2, c2, r2);
 		if(c2 & (HTV_LC_LEFT_ACTIVE | HTV_LC_RIGHT_ACTIVE))
 		{
-			li.sec_prev_kind = r2 >= 0 ? 2 : 1;
-			li.sec_prev_row = r2;
-			li.sec_prev_comp = (((f2 * dp.lines) + l2) & 1) ? 1 : 2;   // a D'r line stores u, a D'b line v
+			o.sec_prev_kind = r2 >= 0 ? 2 : 1;
+			o.sec_prev_row = r2;
+			o.sec_prev_comp = (((f2 * dp.lines) + l2) & 1) ? 1 : 2;   // a D'r line stores u, a D'b line v
 			break;
 		}
 	}
 }
 
-__device__ void line_raster(const htv_dparams_t &dp, const DevTables &dt, int64_t L, LineRaster &li)
+// the VBI overlay on scan line L (dt.ov_line is sorted): m = (replace from, replace to, replace value, row of dt.ov_add
+// or -1); false, and m = (0, 0, 0, -1), on a line without one
+__device__ __forceinline__ bool line_overlay(const DevTables &dt, int64_t L, int4 &m)
 {
-	li.valid = L >= 0;
-	li.nent = 0;
-	li.sec_proc = 0;
-	li.ov_any = 0; li.ov_from = li.ov_to = 0; li.ov_value = 0; li.ov_add = -1;
-	if(dt.ov_n > 0 && L >= 0)
-	{
-		int lo = 0, hi = dt.ov_n - 1;
-		while(lo < hi) { const int mid = (lo + hi) >> 1; if(dt.ov_line[mid] < L) lo = mid + 1; else hi = mid; }
-		if(dt.ov_line[lo] == L)
-		{
-			const int4 m = dt.ov_meta[lo];
-			li.ov_any = 1; li.ov_from = m.x; li.ov_to = m.y; li.ov_value = m.z; li.ov_add = m.w;
-		}
-	}
-	if(dp.colour_mode == HTV_SECAM) line_secam(dp, dt, L, li);
-	if(L < 0) { li.frame = li.line = li.code = li.pal = 0; li.al = li.ar = -1; li.row_off = -1; li.clut_off = 0; return; }
-	const int64_t f0 = L / dp.lines;
-	li.frame = (int) (f0 + 1);
-	li.line = (int) (L - f0 * dp.lines) + 1;
-	li.code = dt.codes[li.line];
-	const int left = li.code & HTV_LC_LEFT_ACTIVE, right = li.code & HTV_LC_RIGHT_ACTIVE;
-	li.al = left ? dp.active_left : (right ? dp.half_width : -1);
-	li.ar = right ? dp.active_left + dp.active_width : (left ? dp.half_width : -1);
+	m = make_int4(0, 0, 0, -1);
+	if(dt.ov_n <= 0 || L < 0) return(false);
+	int lo = 0, hi = dt.ov_n - 1;
+	while(lo < hi) { const int mid = (lo + hi) >> 1; if(dt.ov_line[mid] < L) lo = mid + 1; else hi = mid; }
+	if(dt.ov_line[lo] != L) return(false);
+	m = dt.ov_meta[lo];
+	return(true);
+}
 
-	// source row (ref video.c:2812-2895): a progressive source on an interlaced raster shifts down one row
-	int vy;
-	if(dp.raster == HTV_RASTER_625) vy = li.line < 313 ? (li.line - 23) * 2 : (li.line - 336) * 2 + 1;
-	else vy = li.line < 265 ? (li.line - 23) * 2 : (li.line - 286) * 2 + 1;
-	if(vy >= 0 && dp.interlaced != 0) vy += 1;
-	if(vy < 0 || vy >= dp.active_lines) vy = -1;
-	li.row_off = -1;
-	if(vy >= 0 && dt.frames)
+// Raster descriptors of lines first .. first + n - 1, entry i <-> line first + i, one thread per line: LineS2 rows for
+// SECAM, LineR2 rows for every other colour system
+__global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const DevTables dt, void *out, int64_t first, int n)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= n) return;
+	const int64_t L = first + i;
+	int frame, line, code; long long row_off;
+	line_numbers(dp, dt, L, frame, line, code, row_off);
+	const int left = L >= 0 ? code & HTV_LC_LEFT_ACTIVE : 0, right = L >= 0 ? code & HTV_LC_RIGHT_ACTIVE : 0;
+	const int al = left ? dp.active_left : (right ? dp.half_width : -1);
+	const int ar = right ? dp.active_left + dp.active_width : (left ? dp.half_width : -1);
+	const int tmpl = L < 0 ? dp.lines + 1 : (L == 0 ? dp.lines : line - 1);
+	if(dp.colour_mode == HTV_SECAM)
 	{
-		const int64_t fi = f0 - dt.frame_map_first;
-		if(fi >= 0 && fi < dt.frame_map_len)
-		{
-			const int slot = dt.frame_map[fi];              // -1: the source has no picture (black)
-			if(slot >= 0) li.row_off = ((long long) slot * dp.active_lines + vy) * (long long) dp.active_width;
-		}
+		LineS2 o;
+		o.valid = L >= 0; o.tmpl = tmpl; o.al = al; o.ar = ar;
+		o.keep = dt.tmpl_keep_any[tmpl];
+		o.row_off = row_off;
+		line_secam(dp, dt, L, frame, line, code, o);
+		reinterpret_cast<LineS2 *>(out)[i] = o;
+		return;
 	}
-
-	li.pal = 0;
-	li.clut_off = 0;
-	if(dp.colour_mode == HTV_PAL || dp.colour_mode == HTV_NTSC)
+	LineR2 o;
+	o.valid = L >= 0; o.tmpl = tmpl; o.al = al; o.ar = ar;
+	o.keep = dt.tmpl_keep_any[tmpl];
+	o.pal = 0;
+	o.clut_off = 0;
+	if(L >= 0 && (dp.colour_mode == HTV_PAL || dp.colour_mode == HTV_NTSC))
 	{
-		const int b = (li.code & HTV_LC_BURST_MASK) >> HTV_LC_BURST_SHIFT;
-		li.pal = b == 1 || (b == 2 && (li.frame & 1) == 0) || (b == 3 && (li.frame & 1) == 1);
-		if(dp.colour_mode == HTV_PAL && li.pal && ((li.frame + li.line) & 1)) li.pal = -1;
-		li.clut_off = (unsigned int) (((unsigned long long) L * (unsigned long long) dp.W) % dp.clut_width);
+		const int b = (code & HTV_LC_BURST_MASK) >> HTV_LC_BURST_SHIFT;
+		o.pal = b == 1 || (b == 2 && (frame & 1) == 0) || (b == 3 && (frame & 1) == 1);
+		if(dp.colour_mode == HTV_PAL && o.pal && ((frame + line) & 1)) o.pal = -1;
+		o.clut_off = (unsigned int) (((unsigned long long) L * (unsigned long long) dp.W) % dp.clut_width);
 	}
-
-	// sync pulse pieces landing on this line: the previous line's overrun, its own pulses, and
-	// the next line's leading edge (ref vbidata.c:186-239). Only the last adds inside the picture.
-	int n = 0;
-	for(int s = -1; s <= 1; s++)
-	{
-		const int64_t S = L + s;
-		if(S < 0) continue;
-		const int mask = dt.codes[(int) (S % dp.lines) + 1] & HTV_LC_SYNC_MASK;
-		for(int b = 0; b < 5; b++)
-		{
-			if(!(mask & (1 << b))) continue;
-			const int base = dp.pulse_off[b] + s * dp.W;
-			if(base + dp.pulse_len[b] <= 0 || base >= dp.W || n >= MAX_ENT) continue;
-			li.ent_base[n] = base; li.ent_len[n] = dp.pulse_len[b];
-			li.ent_pos[n] = dp.pulse_pos[b]; li.ent_keep[n] = s == 1;
-			n++;
-		}
-	}
-	li.nent = n;
+	int4 m;
+	o.ov_any = line_overlay(dt, L, m);
+	o.ov_from = m.x; o.ov_to = m.y; o.ov_value = m.z; o.ov_add = m.w;
+	o.row_off = row_off;
+	o.pad = 0;
+	reinterpret_cast<LineR2 *>(out)[i] = o;
 }
 
 // ---------------------------------------------------------------------------
@@ -1044,66 +1019,6 @@ k_line_desc_a2(const __grid_constant__ htv_dparams_t dp, const DevTables dt, Lin
 	}
 }
 
-// raster descriptors: index -1 .. nlines+1 <-> line line0-2 .. line0+nlines
-// SECAM raster in the fused kernel's form (k_sec_raster, htv_secam_raster.cuh): what it needs to know about a line
-struct __align__(16) LineS2 {
-	int valid;                        // 0: before the stream
-	int tmpl;                         // row of the line templates
-	int al, ar;                       // active sample range [al, ar), -1 if none
-	int keep;                         // the template's keep part is non-zero somewhere
-	int sec_proc, sec_dr;             // the line carries a subcarrier; 1: D'r line (uses v), 0: D'b (uses u)
-	int sec_prev_kind;                // what the line-average store holds: 0 zeros, 1 black, 2 a picture row
-	int sec_prev_comp;                // ... and which component of it: 1 u, 2 v
-	int pad0, pad1, pad2;
-	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
-	long long sec_prev_row;           // pixel offset of the stored row
-};
-static_assert(sizeof(LineS2) == 64, "LineS2 is read as four int4");
-
-// the compact descriptor of line L from its full one (written by k_line_desc_r, which describes the same lines for the chain)
-__device__ __forceinline__ void line_s2(const htv_dparams_t &dp, const DevTables &dt, int64_t L, const LineRaster &li, LineS2 &out)
-{
-	LineS2 o;
-	o.valid = li.valid;
-	o.tmpl = L < 0 ? dp.lines + 1 : (L == 0 ? dp.lines : li.line - 1);
-	o.al = li.al; o.ar = li.ar;
-	o.keep = dt.tmpl_keep_any[o.tmpl];
-	o.sec_proc = li.sec_proc; o.sec_dr = li.sec_dr;
-	o.sec_prev_kind = li.sec_prev_kind; o.sec_prev_comp = li.sec_prev_comp;
-	o.pad0 = o.pad1 = o.pad2 = 0;
-	o.row_off = li.row_off; o.sec_prev_row = li.sec_prev_row;
-	out = o;
-}
-
-// s2 (SECAM with k_sec_raster): the same lines once more in that kernel's compact form, s2[i] <-> line line0 - 2 + i
-__global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const DevTables dt, LineRaster *lr, int64_t line0, int nlines, LineS2 *s2)
-{
-	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if(i >= nlines + 3) return;
-	line_raster(dp, dt, line0 - 2 + i, lr[i - 1]);
-	if(s2) line_s2(dp, dt, line0 - 2 + i, lr[i - 1], s2[i]);
-}
-
-// the same for the fused line kernel (htv_line.cuh): compact descriptors, index 0 .. nlines+1 <-> line line0-1 .. line0+nlines
-__global__ void k_line_desc_r2(const __grid_constant__ htv_dparams_t dp, const DevTables dt, LineR2 *out, int64_t line0, int nlines)
-{
-	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if(i >= nlines + 2) return;
-	const int64_t L = line0 - 1 + i;
-	LineRaster li;
-	line_raster(dp, dt, L, li);
-	LineR2 o;
-	o.valid = li.valid;
-	o.tmpl = L < 0 ? dp.lines + 1 : (L == 0 ? dp.lines : li.line - 1);
-	o.al = li.al; o.ar = li.ar; o.pal = li.pal;
-	o.keep = dt.tmpl_keep_any[o.tmpl];
-	o.ov_any = li.ov_any; o.ov_from = li.ov_from; o.ov_to = li.ov_to; o.ov_value = li.ov_value; o.ov_add = li.ov_add;
-	o.clut_off = li.clut_off;
-	o.row_off = li.row_off;
-	o.pad = 0;
-	out[i] = o;
-}
-
 __device__ __forceinline__ int round_away(double v)
 {
 	// round() (half away from zero) from the round-to-nearest-even conversion
@@ -1201,7 +1116,7 @@ __device__ __forceinline__ void chroma_fir4(const htv_dparams_t &dp, const int *
 // ---------------------------------------------------------------------------
 
 __global__ void __launch_bounds__(384, 4)
-k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, int16_t *comp, int *comp32,
+k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lr, int16_t *comp, int *comp32,
 	uint8_t *planes, size_t plane_stride, int plane_pitch)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -1210,14 +1125,10 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 	const int UW = W4 + 2 * UOFF;
 	int *su = reinterpret_cast<int *>(smem_raw);                    // index = x + UOFF
 	int *sv = su + UW;
-	__shared__ LineRaster li;
+	__shared__ LineR2 li;
 	const int tid = threadIdx.x;
 
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(lr + blockIdx.x);
-		int4 *dst = reinterpret_cast<int4 *>(&li);
-		if(tid < (int) (sizeof(LineRaster) / 16)) dst[tid] = __ldg(src + tid);
-	}
+	if(tid < 4) reinterpret_cast<int4 *>(&li)[tid] = __ldg(reinterpret_cast<const int4 *>(lr + blockIdx.x) + tid);
 	if(tid < 2 * UOFF)
 	{
 		// U,V outside the line read as zero (the reference filters each line on its own)
@@ -1230,32 +1141,20 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 	int val[SPT];
 	if(x0 < W)
 	{
-		// ---- blanking / luma, unfiltered U,V ----------------------------------
+		// ---- blanking and sync from the line template, luma, unfiltered U,V ------
+		const int trow = li.tmpl * W;
 		int uu[SPT], vv[SPT];
 		#pragma unroll
 		for(int k = 0; k < SPT; k++)
 		{
 			const int x = x0 + k;
-			val[k] = li.valid ? dp.blank : 0; uu[k] = 0; vv[k] = 0;
+			val[k] = x < W ? __ldg(dt.tmpl_out + trow + x) : 0; uu[k] = 0; vv[k] = 0;
 			if(x >= li.al && x < li.ar)
 			{
 				const unsigned int rgb = li.row_off >= 0 ? (__ldg(dt.frames + li.row_off + (x - dp.active_left)) & 0xFFFFFF) : 0;
 				yuv_lookup(dt, rgb, val[k], uu[k], vv[k]);
+				if(li.keep) val[k] += __ldg(dt.tmpl_keep + trow + x);       // the next line's leading edge
 				if(!li.pal) uu[k] = vv[k] = 0;
-			}
-		}
-		// ---- sync pulse pieces landing on this line -----------------------------
-		for(int e = 0; e < li.nent; e++)
-		{
-			const int d0 = x0 - li.ent_base[e];
-			if(d0 + SPT - 1 < 0 || d0 >= li.ent_len[e]) continue;
-			#pragma unroll
-			for(int k = 0; k < SPT; k++)
-			{
-				const int d = d0 + k, x = x0 + k;
-				if(d < 0 || d >= li.ent_len[e] || x >= W) continue;
-				if(!li.ent_keep[e] && x >= li.al && x < li.ar) continue;   // overwritten by the picture
-				val[k] += __ldg(dt.pulse_values + li.ent_pos[e] + d);
 			}
 		}
 		if(li.pal)
@@ -1407,7 +1306,7 @@ MMA_I8(mma_us, "u8", "s8")
 MMA_I8(mma_uu, "u8", "u8")
 
 __global__ void __launch_bounds__(384, 3)
-k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, int16_t *comp, SecScratch ss)
+k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, int16_t *comp, SecScratch ss)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = dp.W;
@@ -1418,14 +1317,10 @@ k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, con
 	// luma as high / low byte planes for the notch on the tensor cores: byte i = sample i - MF_LEAD, zero outside 0 .. W-1
 	const int RBn = mf_row_bytes(W);
 	unsigned char *pl = reinterpret_cast<unsigned char *>(cbin + W4 + 32);
-	__shared__ LineRaster li;
+	__shared__ LineS2 li;
 	const int tid = threadIdx.x;
 
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(lr + blockIdx.x);
-		int4 *dst = reinterpret_cast<int4 *>(&li);
-		if(tid < (int) (sizeof(LineRaster) / 16)) dst[tid] = __ldg(src + tid);
-	}
+	if(tid < 4) reinterpret_cast<int4 *>(&li)[tid] = __ldg(reinterpret_cast<const int4 *>(lr + blockIdx.x) + tid);
 	for(int i = tid; i < LOFF; i += blockDim.x) { line[i] = 0; line[W4 + LOFF + i] = 0; }
 	if(tid < 16) { cbin[tid < 8 ? tid : W4 + tid] = 0; }
 	if(dt.notch_atab)
@@ -1444,7 +1339,7 @@ k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, con
 		for(int k = 0; k < SPT; k++)
 		{
 			const int x = x0 + k;
-			val[k] = li.valid ? dp.blank : 0;
+			val[k] = 0;
 			cbv[k] = cur == 1 ? dp.black_u : dp.black_v;
 			int y = 0, u = 0, v = 0;
 			const bool inpic = x >= dp.active_left && x < dp.active_left + dp.active_width;
@@ -1469,25 +1364,20 @@ k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, con
 				cbv[k] = ((cur == 1 ? u : v) + st) / 2;
 			}
 		}
-		for(int e = 0; e < li.nent; e++)
-		{
-			const int d0 = x0 - li.ent_base[e];
-			if(d0 + SPT - 1 < 0 || d0 >= li.ent_len[e]) continue;
-			#pragma unroll
-			for(int k = 0; k < SPT; k++)
-			{
-				const int d = d0 + k, x = x0 + k;
-				if(d < 0 || d >= li.ent_len[e] || x >= W) continue;
-				if(!li.ent_keep[e] && x >= li.al && x < li.ar) continue;
-				val[k] += __ldg(dt.pulse_values + li.ent_pos[e] + d);
-			}
-		}
+		// blanking and sync from the line template (the samples from W to W4 are zero)
+		const int trow = li.tmpl * W;
 		unsigned ph4 = 0, pl4 = 0;
 		#pragma unroll
 		for(int k = 0; k < SPT; k++)
 		{
 			const int x = x0 + k;
-			const int lv = x < W ? wrap16i(val[k]) : 0;
+			int lv = 0;
+			if(x < W)
+			{
+				const bool act = x >= li.al && x < li.ar;
+				lv = act ? val[k] : __ldg(dt.tmpl_out + trow + x);
+				if(act && li.keep) lv = wrap16i(lv + __ldg(dt.tmpl_keep + trow + x));
+			}
 			line[x + LOFF] = lv;
 			cbin[x + 8] = x < W ? cbv[k] : 0;
 			// the notch reads samples left of the picture as zero (ref fir.c:357-375)
@@ -1613,18 +1503,19 @@ k_raster_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, con
 #include "htv_secam.cuh"
 
 // SECAM: the VBI stages sit behind the SECAM stage (ref video.c:4211-4357), so an overlay line is
-// folded in once k_sec_out has added the line's subcarrier to the composite row: replace / add in place. One CTA per row, a handful of rows per frame do work.
-__global__ void __launch_bounds__(256) k_overlay_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, int16_t *comp)
+// folded in once k_sec_out has added the line's subcarrier to the composite row: replace / add in place. One CTA per row
+// (row 0 is scan line line_r0), a handful of rows per frame do work.
+__global__ void __launch_bounds__(256) k_overlay_secam(const __grid_constant__ htv_dparams_t dp, const DevTables dt, int64_t line_r0, int16_t *comp)
 {
-	const LineRaster &li = lr[blockIdx.x];
-	if(!li.ov_any) return;
+	int4 m;
+	if(!line_overlay(dt, line_r0 + blockIdx.x, m)) return;
 	const int W = dp.W;
 	const size_t o = (size_t) blockIdx.x * W;
 	for(int x = threadIdx.x; x < W; x += blockDim.x)
 	{
 		int v = comp[o + x];
-		if(x >= li.ov_from && x < li.ov_to) v = li.ov_value;
-		if(li.ov_add >= 0) v += dt.ov_add[(size_t) li.ov_add * W + x];
+		if(x >= m.x && x < m.y) v = m.z;
+		if(m.w >= 0) v += dt.ov_add[(size_t) m.w * W + x];
 		comp[o + x] = (int16_t) v;
 	}
 }
@@ -2468,7 +2359,7 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	else if(dp.have_fmv) p->path = PATH_FMV;
 	else if(t->rs_taps) p->path = PATH_RS;
 	else if(secam && !sw.split) p->path = PATH_SEC_LINE;
-	else if(!secam && !sw.split && chroma_ok && (!dp.vf_type || mma) && t->tmpl_out) p->path = PATH_LINE;
+	else if(!secam && !sw.split && chroma_ok && (!dp.vf_type || mma)) p->path = PATH_LINE;
 	else p->path = PATH_SPLIT;
 
 	p->raster_smem = sizeof(int) * 2 * (W4 + 2 * UOFF);
@@ -2506,7 +2397,7 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 		p->kl = kfind(kl_tab, miss, [&](const KLine &k) {
 			return(k.vf == vf && k.hq == hq && k.full == full && !k.csat && k.maxt == maxt && k.src && k.snd == -1 && !k.wc && k.st == kst); });
 		// the raster with the luma notch on the tensor cores (k_sec_raster); HTV_FIR=scalar: k_raster_secam
-		if(!sw.scalar && t->tmpl_out)
+		if(!sw.scalar)
 		{
 			p->ks = kfind(ks_tab, miss, [&](const KSec &k) { return(k.full == full && k.maxt == maxt); });
 			p->ks_smem = 2 * sizeof(LineS2) + 4 * rowb + 4 * uvb + sizeof(uint4) * (MF_KSTEPS * 2 * 32 + 64) + 64;
@@ -2629,7 +2520,6 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	DevTables &dt = d->dt;
 
 	dt.codes = (const uint16_t *) dev_copy(d, t->codes, sizeof(uint16_t) * t->ncodes);
-	dt.pulse_values = (const int16_t *) dev_copy(d, t->pulse_values, sizeof(int16_t) * (t->npulse_values + 8));
 	dt.tmpl_out = (const int16_t *) dev_copy(d, t->tmpl_out, sizeof(int16_t) * (size_t) t->tmpl_rows * t->dp.W);
 	dt.tmpl_keep = (const int16_t *) dev_copy(d, t->tmpl_keep, sizeof(int16_t) * (size_t) t->tmpl_rows * t->dp.W);
 	dt.tmpl_keep_any = (const uint8_t *) dev_copy(d, t->tmpl_keep_any, t->tmpl_rows);
@@ -2820,7 +2710,7 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	// the side streams may still be ahead of the caller's; nothing of this encoder is freed under running work
 	cudaDeviceSynchronize();
 	for(int i = 0; i < d->nalloc; i++) cudaFree(d->alloc[i]);
-	cudaFree(d->d_desc_r); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
+	cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
 	if(d->h_map) cudaFreeHost(d->h_map);
 	if(d->h_ov_line) { cudaFreeHost(d->h_ov_line); cudaFreeHost(d->h_ov_meta); cudaFreeHost(d->h_ov_add); }
 	cudaFree(d->d_ov_line); cudaFree(d->d_ov_meta); cudaFree(d->d_ov_add);
@@ -3047,6 +2937,28 @@ static int launch_desc_a2(htv_dev_t *d, LineA2 *la, int64_t line0, int n, cudaSt
 	return(HTV_OK);
 }
 
+// The descriptor buffers of calls of up to n lines: raster descriptors (LineS2 for SECAM, else LineR2) where the context
+// rasters, sound descriptors where it modulates, two of each for the fused line kernel. Growing them first waits for
+// every stream that may still read the old ones.
+static int desc_reserve(htv_dev_t *d, int n, cudaStream_t st)
+{
+	if(n <= d->desc_cap) return(HTV_OK);
+	const DevPlan &p = d->plan;
+	const size_t bufs = p.path == PATH_LINE ? 2 : 1;
+	cudaStreamSynchronize(st);
+	cudaStreamSynchronize(d->side);
+	cudaStreamSynchronize(d->side2);
+	cudaStreamSynchronize(d->side3);
+	cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
+	d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
+	d->desc_cap = 0;
+	if(d->dp.colour_mode == HTV_SECAM) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) n + 3)));
+	else if(p.path != PATH_RS) CK(cudaMalloc(&d->d_desc_r2, bufs * sizeof(LineR2) * ((size_t) n + 2)));
+	if(p.path != PATH_RASTER) CK(cudaMalloc(&d->d_desc_a2, bufs * sizeof(LineA2) * ((size_t) n + 1)));
+	d->desc_cap = n;
+	return(HTV_OK);
+}
+
 // The plan's split modulator over n lines (htv_dev_render_lines, htv_dev_render_lines_rs): descriptors la, the composite
 // stream as k_raster / k_resample left it for this modulator (byte planes, int32, or the int16 `comp`), output o
 static void launch_mod(const htv_dev_t *d, int n, const LineA2 *la, const int16_t *comp, int16_t *o, const int16_t *acc,
@@ -3069,22 +2981,8 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 	if(nlines <= 0) return(HTV_OK);
 	// FM video with a pre-emphasis filter: the modulator also integrates the pipeline's fill line
 	const int fm_skip = d->dp.have_fmv && d->dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
-	if(nlines > d->desc_cap)
-	{
-		cudaStreamSynchronize(st);
-		cudaStreamSynchronize(d->side);
-		cudaStreamSynchronize(d->side2);
-		cudaStreamSynchronize(d->side3);
-		cudaFree(d->d_desc_r); cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
-		d->d_desc_r = d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
-		d->desc_cap = 0;
-		if(p.path == PATH_LINE) CK(cudaMalloc(&d->d_desc_r2, 2 * sizeof(LineR2) * ((size_t) nlines + 2)));
-		else CK(cudaMalloc(&d->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 3)));
-		CK(cudaMalloc(&d->d_desc_a2, (p.path == PATH_LINE ? 2 : 1) * sizeof(LineA2) * ((size_t) nlines + 1)));
-		if(p.ks) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) nlines + 3)));
-		d->desc_cap = nlines;
-	}
-	LineRaster *lr0 = (LineRaster *) d->d_desc_r + 1;
+	if(desc_reserve(d, nlines, st) != HTV_OK) return(HTV_ERROR);
+	const bool secam = d->dp.colour_mode == HTV_SECAM;
 	if(p.path == PATH_LINE)
 	{
 		// one persistent launch for the whole call: every CTA walks its own run of consecutive lines
@@ -3093,12 +2991,12 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		if(d->ahead && d->r2_armed)
 		{
 			// behind the frame map on side3 (htv_dev_set_frame_map); overlays were staged by the host before this call
-			k_line_desc_r2<<<(nlines + 2 + 63) / 64, 64, 0, d->side3>>>(dp, d->dt, lr2, line0, nlines);
+			k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, d->side3>>>(dp, d->dt, lr2, line0 - 1, nlines + 2);
 			CK(cudaEventRecord(d->ev_r2, d->side3));
 			CK(cudaStreamWaitEvent(st, d->ev_r2, 0));
 			d->r2_armed = 0;
 		}
-		else k_line_desc_r2<<<(nlines + 2 + 63) / 64, 64, 0, st>>>(dp, d->dt, lr2, line0, nlines);
+		else k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, st>>>(dp, d->dt, lr2, line0 - 1, nlines + 2);
 		if(!d->side_armed)
 		{
 			CK(cudaEventRecord(d->ev_in, st));
@@ -3139,7 +3037,11 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		CK(cudaGetLastError());
 		return(HTV_OK);
 	}
-	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, lr0, line0, nlines, p.ks ? (LineS2 *) d->d_desc_s2 : NULL);
+	// raster descriptors: SECAM's ls0[i] <-> line line0 - 2 + i (its rows reach one line further back), lr0[i] <-> line line0 - 1 + i
+	const LineS2 *ls0 = (const LineS2 *) d->d_desc_s2;
+	const LineR2 *lr0 = (const LineR2 *) d->d_desc_r2;
+	if(secam) k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, d->d_desc_s2, line0 - 2, nlines + 3);
+	else k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, d->d_desc_r2, line0 - 1, nlines + 2);
 	d->launches++;
 	// la2[i] <-> line line0 - fm_skip + i
 	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
@@ -3154,14 +3056,13 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
 		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * d->dp.W * (d->dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
-		if(d->dp.colour_mode == HTV_SECAM)
+		if(secam)
 		{
 			// rows 0 .. n+2 <-> lines first-2 .. first+n; the chain covers rows 0 .. n+1
-			const LineRaster *lr = lr0 + done - 1;
+			const LineS2 *ls = ls0 + done;
 			if(p.ks)
 			{
-				// rows 0 .. n+2: their own compact descriptors, then runs of rows per persistent CTA
-				const LineS2 *ls = (const LineS2 *) d->d_desc_s2 + done;
+				// rows 0 .. n+2 in runs of rows per persistent CTA
 				const int nr = n + 3;
 				int run = (nr + d->kl_ctas - 1) / d->kl_ctas;
 				if(run < 4) run = 4;
@@ -3169,7 +3070,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				p.ks->fn<<<grid, p.kl_threads, p.ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec);
 				d->launches++;
 			}
-			else k_raster_secam<<<n + 3, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, lr, d->d_comp, d->sec);
+			else k_raster_secam<<<n + 3, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, ls, d->d_comp, d->sec);
 			// the chain (htv_secam.cuh): pass 0 over every line, the predictor, then refinement passes until no line's
 			// outgoing state changes - at that fixed point every line was computed from its true predecessor state =
 			// the sequential result. The loop needs the change count on the host, so SECAM launches synchronise.
@@ -3186,16 +3087,16 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				cudaMemsetAsync(d->sec.flags, 0, sizeof(int) * 4, st);
 				if(pass == 0)
 				{
-					k_sec_pass0<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, nch);
+					k_sec_pass0<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch);
 					// propose the states pass 1 starts from (see k_sec_predict); st[0] takes them over
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, d->sec_pred);
+					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
 					cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 					d->launches += 2;
 					continue;
 				}
-				k_sec_refine<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, pass);
-				k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, lr, d->sec, pass, d->sec_many);
-				k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, lr, d->sec, pass, d->sec_many);
+				k_sec_refine<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, pass);
+				k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
+				k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
 				d->launches += 3;
 				CK(cudaMemcpyAsync(fl, d->sec.flags, sizeof(fl), cudaMemcpyDeviceToHost, st));
 				CK(cudaStreamSynchronize(st));
@@ -3218,7 +3119,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 					repredict--;
 					if(pass & 1) cs.repredict_odd++; else cs.repredict_even++;
 					if(pass & 1) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, lr, d->sec, nch, d->sec_pred);
+					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
 					if(!(pass & 1)) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 					d->launches++;
 				}
@@ -3230,12 +3131,12 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int
 				return(HTV_ERROR);
 			}
 			if((pass - 1) & 1) cs.final_odd++; else cs.final_even++;
-			k_sec_carry<<<1, 32, 0, st>>>(lr, d->sec, n - 1, pass - 1);
-			k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, lr, d->sec, d->d_comp, nch);
+			k_sec_carry<<<1, 32, 0, st>>>(ls, d->sec, n - 1, pass - 1);
+			k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, ls, d->sec, d->d_comp, nch);
 			d->launches += 2;
 			if(d->dt.ov_n > 0)
 			{
-				k_overlay_secam<<<n + 3, 256, 0, st>>>(d->dp, d->dt, lr, d->d_comp);
+				k_overlay_secam<<<n + 3, 256, 0, st>>>(d->dp, d->dt, line0 + done - 2, d->d_comp);
 				d->launches++;
 			}
 			cstream = d->d_comp + d->dp.W;          // k_mod's line b sits at row b + 2
@@ -3331,31 +3232,12 @@ extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0
 	if(nlines <= 0) return(HTV_OK);
 	const DevPlan &p = d->plan;
 	if(p.path != PATH_RS || r->plan.path != PATH_RASTER || p.plane_pitch || (d->dp.W & 3)) return(HTV_ERROR);
-	if(nlines > d->desc_cap)
-	{
-		cudaStreamSynchronize(st);
-		cudaStreamSynchronize(d->side);
-		cudaStreamSynchronize(d->side2);
-		cudaFree(d->d_desc_a2);
-		d->d_desc_a2 = NULL;
-		d->desc_cap = 0;
-		CK(cudaMalloc(&d->d_desc_a2, sizeof(LineA2) * ((size_t) nlines + 1)));
-		d->desc_cap = nlines;
-	}
-	if(nlines + 1 > r->desc_cap)
-	{
-		cudaStreamSynchronize(st);
-		cudaFree(r->d_desc_r);
-		r->d_desc_r = NULL;
-		r->desc_cap = 0;
-		CK(cudaMalloc(&r->d_desc_r, sizeof(LineRaster) * ((size_t) nlines + 4)));
-		r->desc_cap = nlines + 1;
-	}
-	// raster descriptors for lines line0 - 2 .. line0 + nlines + 1 (one line more than without a resampler:
-	// the emitted line t is resampled line t + 1 and the video filter looks into t + 2)
-	LineRaster *lr0 = (LineRaster *) r->d_desc_r + 1;
+	if(desc_reserve(d, nlines, st) != HTV_OK || desc_reserve(r, nlines + 1, st) != HTV_OK) return(HTV_ERROR);
+	// raster descriptors lr0[i] <-> line line0 - 1 + i for lines line0 - 1 .. line0 + nlines + 1 (one line more than
+	// without a resampler: the emitted line t is resampled line t + 1 and the video filter looks into t + 2)
+	const LineR2 *lr0 = (const LineR2 *) r->d_desc_r2;
 	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
-	k_line_desc_r<<<(nlines + 4 + 63) / 64, 64, 0, st>>>(r->dp, r->dt, lr0, line0, nlines + 1, NULL);
+	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(r->dp, r->dt, r->d_desc_r2, line0 - 1, nlines + 3);
 	d->launches++;
 	if(launch_desc_a2(d, la2, line0, nlines, st) != HTV_OK) return(HTV_ERROR);
 	bool joined = false;

@@ -31,7 +31,7 @@ __device__ __forceinline__ size_t sec_t(const SecScratch &ss, int c, int x) { re
 
 // state handed to row c: the outgoing state of the nearest row before it that carries a subcarrier (rows without
 // one pass the state on, the two field-start lines clear A and B: ref video.c:3149-3160), or the launch's carry
-__device__ __forceinline__ SecState sec_incoming(const LineRaster *lr, const SecScratch &ss, int c, const SecState *prev_out, int &from)
+__device__ __forceinline__ SecState sec_incoming(const LineS2 *lr, const SecScratch &ss, int c, const SecState *prev_out, int &from)
 {
 	bool clr = false;
 	int p = c - 1;
@@ -153,7 +153,7 @@ struct SecTailIn {
 };
 
 template<bool AL>
-__device__ __forceinline__ void sec_tail_load(const htv_dparams_t &dp, const LineRaster &li, const SecScratch &ss, int c, SecTailIn &ti)
+__device__ __forceinline__ void sec_tail_load(const htv_dparams_t &dp, const LineS2 &li, const SecScratch &ss, int c, SecTailIn &ti)
 {
 	const int W = dp.W, ck = AL ? W - 8 : sec_ck(W);
 	sec_unpack8(*reinterpret_cast<const int4 *>(ss.cbT + sec_t(ss, c, ck)), ti.cbv);
@@ -219,7 +219,7 @@ __device__ __forceinline__ SecState sec_tail_core(const htv_dparams_t &dp, const
 	return(out);
 }
 
-__device__ __forceinline__ SecState sec_tail(const htv_dparams_t &dp, const DevTables &dt, const LineRaster &li, const SecScratch &ss,
+__device__ __forceinline__ SecState sec_tail(const htv_dparams_t &dp, const DevTables &dt, const LineS2 &li, const SecScratch &ss,
 	int c, const SecState &in, const SecChk &ck4, bool store)
 {
 	SecTailIn ti;
@@ -236,12 +236,12 @@ __device__ __forceinline__ SecState sec_tail(const htv_dparams_t &dp, const DevT
 // line leaves when started from rest SEC_WARMUP samples before its end. IIR and FM recurrence run a group apart in
 // the same thread: the FM look-ups of group g are in flight while the IIR does group g + 1.
 __global__ void __launch_bounds__(32)
-k_sec_pass0(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int n)
+k_sec_pass0(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int n)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	if(c >= n) return;
 	const int W = dp.W, ck = sec_ck(W), G0 = ck >> 3;
-	const LineRaster &li = lr[c];
+	const LineS2 &li = lr[c];
 	SecState *cur = ss.st[0];
 	int from;
 	SecState in = sec_incoming(lr, ss, c, ss.st[1], from);
@@ -304,7 +304,7 @@ k_sec_pass0(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const 
 #define SEC_PRED_HALO 16
 #define SEC_PRED_T 256
 template<bool AL>
-__device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const DevTables &dt, const LineRaster *lr, const SecScratch &ss, int n, int iters,
+__device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const DevTables &dt, const LineS2 *lr, const SecScratch &ss, int n, int iters,
 	SecState (*sm)[SEC_PRED_T])
 {
 	const int tid = threadIdx.x;
@@ -320,7 +320,7 @@ __device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const 
 	above = s;
 	if(live)
 	{
-		const LineRaster &li = lr[c];
+		const LineS2 &li = lr[c];
 		proc = li.sec_proc != 0; clear = li.sec_clear != 0;
 		s = src[c];
 		if(proc) { sec_tail_load<AL>(dp, li, ss, c, ti); k4 = ss.chk[c]; }
@@ -346,7 +346,7 @@ __device__ __forceinline__ void sec_predict_body(const htv_dparams_t &dp, const 
 }
 
 __global__ void __launch_bounds__(SEC_PRED_T)
-k_sec_predict(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int n, int iters)
+k_sec_predict(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int n, int iters)
 {
 	__shared__ SecState sm[2][SEC_PRED_T];
 	if((dp.W & 7) == 0) sec_predict_body<true>(dp, dt, lr, ss, n, iters, sm);
@@ -358,12 +358,12 @@ k_sec_predict(const __grid_constant__ htv_dparams_t dp, const DevTables dt, cons
 // rounded outputs that differ are rewritten, the first one inside the FM range is remembered. Then the FM recurrence:
 // from the checkpoint before ck when nothing ahead of it changed (the usual case), else the line goes on the list.
 __global__ void __launch_bounds__(32)
-k_sec_refine(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int n, int pass)
+k_sec_refine(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int n, int pass)
 {
 	const int c = blockIdx.x * blockDim.x + threadIdx.x;
 	if(c >= n) return;
 	const int W = dp.W, ck = sec_ck(W), G0 = ck >> 3;
-	const LineRaster &li = lr[c];
+	const LineS2 &li = lr[c];
 	const SecState *prev = ss.st[(pass + 1) & 1];
 	SecState *cur = ss.st[pass & 1];
 	int from;
@@ -443,7 +443,7 @@ k_sec_refine(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const
 #define SEC_LIST_MANY 2048             // above this many lines a thread per line has the better throughput (k_sec_fm_list_t)
 // `many`: that threshold, an argument of both list kernels (HTV_SEC=list=warp / thread moves it past either end)
 __global__ void __launch_bounds__(32 * SEC_LIST_WARPS)
-k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass, int many)
+k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int pass, int many)
 {
 	const int lane = threadIdx.x & 31;
 	const int nw = gridDim.x * SEC_LIST_WARPS, count = ss.flags[3];
@@ -454,7 +454,7 @@ k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, cons
 	for(int i = blockIdx.x * SEC_LIST_WARPS + (threadIdx.x >> 5); i < count; i += nw)
 	{
 		const int c = ss.list[i];
-		const LineRaster &li = lr[c];
+		const LineS2 &li = lr[c];
 		const int sr = li.sec_sr, lim = min(sr, ck);
 		const int dmin = dp.secam_dmin[li.sec_dr], dmax = dp.secam_dmax[li.sec_dr];
 		int pi = li.sec_sign > 0 ? 2147483647 : -2147483647, pq = 0;
@@ -515,14 +515,14 @@ k_sec_fm_list(const __grid_constant__ htv_dparams_t dp, const DevTables dt, cons
 // one THREAD per listed line, 32 listed lines per warp - pass 0's arrangement, on the compacted list. FM inputs are
 // loaded two groups ahead, their look-ups issued one group ahead of the recurrence.
 __global__ void __launch_bounds__(32)
-k_sec_fm_list_t(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int pass, int many)
+k_sec_fm_list_t(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int pass, int many)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	const int count = ss.flags[3];
 	if(count <= many || i >= count) return;
 	const int c = ss.list[i];
 	const int W = dp.W, ck = sec_ck(W), G0 = ck >> 3;
-	const LineRaster &li = lr[c];
+	const LineS2 &li = lr[c];
 	const SecState *prev = ss.st[(pass + 1) & 1];
 	SecState *cur = ss.st[pass & 1];
 	const int sl = dp.burst_left, sr = li.sec_sr, lim = min(sr, ck);
@@ -553,7 +553,7 @@ k_sec_fm_list_t(const __grid_constant__ htv_dparams_t dp, const DevTables dt, co
 }
 
 // carry for the next launch: the state after chain row `idx` of the final pass (rows without a subcarrier pass it on)
-__global__ void k_sec_carry(const LineRaster *lr, SecScratch ss, int idx, int pass_final)
+__global__ void k_sec_carry(const LineS2 *lr, SecScratch ss, int idx, int pass_final)
 {
 	if(threadIdx.x == 0 && blockIdx.x == 0)
 	{
@@ -567,7 +567,7 @@ __global__ void k_sec_carry(const LineRaster *lr, SecScratch ss, int idx, int pa
 // video.c:3216-3228) - added to the composite rows in place, for 32 lines x 64 samples per CTA: read from the transposed
 // arrays lane = line, exchanged through shared memory, added row-wise.
 __global__ void __launch_bounds__(256)
-k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineRaster *lr, SecScratch ss, int16_t *comp, int nchain)
+k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int16_t *comp, int nchain)
 {
 	__shared__ __align__(16) short tile[32][64 + 8];
 	__shared__ int any[32];
@@ -582,7 +582,7 @@ k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 		for(int k = 0; k < 8; k++) o[k] = 0;
 		if(c < nchain && xb < W)
 		{
-			const LineRaster &li = lr[c];
+			const LineS2 &li = lr[c];
 			const int top = min(li.sec_sr, W);
 			if(li.sec_proc && li.valid && xb + 8 > sl && xb < top)              // fill lines are never emitted
 			{

@@ -3,8 +3,8 @@
 // What k_raster_secam does one CTA per line and one thread per 4 consecutive samples - luma from template + picture,
 // the colour-difference baseband averaged with the line above (ref video.c:3093-3147), the 51-tap luma notch over the
 // picture (ref video.c:3082-3090) and the 15-tap baseband low-pass (ref video.c:3162-3180) - a persistent CTA does here
-// for a run of lines in k_line's lane layout (lane (g, t) of warp nt owns samples 128 nt + 32 t + g + 8 j): the line
-// template replaces the sync-pulse entries, both filters are byte-split int8 contractions on the tensor cores whose
+// for a run of lines in k_line's lane layout (lane (g, t) of warp nt owns samples 128 nt + 32 t + g + 8 j): both
+// filters are byte-split int8 contractions on the tensor cores whose
 // accumulators land on the lane's own four samples, the next line's template and pixels are fetched while this line's
 // filters run, and there is one barrier per line (byte planes double-buffered). Lines do not depend on each other.
 // Outputs as before: composite rows (int16, luma only - k_sec_out adds the subcarrier), the baseband in the chain's

@@ -252,8 +252,9 @@ static int build_pulse(int16_t *dst, int32_t *off, double offset, double width, 
  *   tmpl_keep[row][x]  the part that is also added INSIDE the picture (the picture overwrites the line's
  *                      own and the previous line's pieces; only the next line's edge comes later)
  * row = line - 1 for lines 1 .. lines; row `lines` = line 1 of the very first frame (nothing before it);
- * row lines + 1 = before the stream (zeros). int16 wrap-around sums, as the reference's line buffer. */
-static void build_templates(struct htv_tables_t *t)
+ * row lines + 1 = before the stream (zeros). int16 wrap-around sums, as the reference's line buffer.
+ * Every raster kernel takes its blanking and sync from here. -1: out of memory. */
+static int build_templates(struct htv_tables_t *t)
 {
 	const htv_dparams_t *dp = &t->dp;
 	const int W = dp->W, nl = dp->lines, rows = nl + 2;
@@ -262,6 +263,7 @@ static void build_templates(struct htv_tables_t *t)
 	t->tmpl_out = calloc((size_t) rows * W, sizeof(int16_t));
 	t->tmpl_keep = calloc((size_t) rows * W, sizeof(int16_t));
 	t->tmpl_keep_any = calloc(rows, 1);
+	if(!t->pulse_values || !t->tmpl_out || !t->tmpl_keep || !t->tmpl_keep_any) return(-1);
 	for(r = 0; r <= nl; r++)
 	{
 		const int line0 = r == nl ? 0 : r;                 /* 0-based line within the frame */
@@ -292,6 +294,7 @@ static void build_templates(struct htv_tables_t *t)
 			}
 		}
 	}
+	return(0);
 }
 
 /* ---- the build --------------------------------------------------------- */
@@ -438,7 +441,12 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 	}
 
 	build_codes(t);
-	build_templates(t);
+	if(build_templates(t) != 0)
+	{
+		fprintf(stderr, "hacktv_b200: out of memory for the line templates\n");
+		htv_tables_free(t);
+		return(NULL);
+	}
 
 	if(c->colour_mode == HTV_PAL || c->colour_mode == HTV_NTSC)
 	{

@@ -48,6 +48,14 @@ CASES = [
     ("i_16M_filter_split_long", "i", dict(vfilter=True), 16_000_000, 0, SPLIT, "int16", 20_500),
     ("i_16M_filter_default", "i", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
     ("l_16M_filter_default", "l", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
+    # SECAM: k_raster_secam + chain + k_line<SRC>; the same behind the split modulator; at 13.5 Msps the chain's
+    # work-list kernels run; baseband (no video filter)
+    ("l_16M_filter_scalar", "l", dict(vfilter=True), 16_000_000, 0, dict(HTV_FIR="scalar"), "int16", 1400),
+    ("l_16M_filter_split_scalar", "l", dict(vfilter=True), 16_000_000, 0, dict(SPLIT, HTV_FIR="scalar"), "int16", 1400),
+    ("l_13M5_filter_default", "l", dict(vfilter=True), 13_500_000, 0, {}, "int16", 1400),
+    ("secam_16M", "secam", dict(), 16_000_000, 0, {}, "int16", 1400),
+    ("pal_16M_from_13M5", "pal", dict(), 16_000_000, 13_500_000, {}, "int16", 1400),
+    ("i_16M_from_14M_filter", "i", dict(vfilter=True), 16_000_000, 14_000_000, {}, "int16", 1400),
 ]
 
 # split render_add: the second channel added into the first one's stream
@@ -55,7 +63,7 @@ ADD_CASE = ("i_16M_filter_split_render_add", "i", dict(vfilter=True, offset=-3_0
             dict(vfilter=True, offset=2_500_000, level=0.5), 16_000_000, SPLIT, 1400)
 
 TIMED = ["i_16M_filter_split_mma", "i_16M_filter_split_tma", "pal-fm_20M", "pal-fm_20M_filter",
-         "i_16M_from_13M5_filter", "i_16M_from_13M5", "l_16M_filter_split", "i_10M_split"]
+         "i_16M_from_13M5_filter", "i_16M_from_13M5", "l_16M_filter_split", "i_10M_split", "l_16M_filter_default"]
 
 
 def card():
