@@ -586,8 +586,7 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 			if(acc_lines < 0) return(HTV_ERROR);
 			acc = s->pt_dev;
 		}
-		if(s->rdev != s->dev) r = htv_dev_render_lines_rs(s->dev, s->rdev, L0, n, d_out, acc, acc_lines, stream);
-		else r = htv_dev_render_lines(s->dev, L0, n, d_out, acc, acc_lines, stream);
+		r = htv_dev_render_lines(s->dev, s->rdev != s->dev ? s->rdev : NULL, L0, n, d_out, acc, acc_lines, stream);
 		if(r != HTV_OK) return(r);
 	}
 	s->next_line += n;

@@ -152,11 +152,9 @@ extern int htv_dev_set_frame_map(htv_dev_t *d, const int32_t *slot_of_frame, int
 extern int htv_dev_upload_audio(htv_dev_t *d, int64_t j0, const int16_t *pcm, size_t npairs, void *stream);
 /* audio-rate pre-pass for the absolute audio-clock sample range [m0, m1) */
 extern int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void *stream);
-/* the line kernel(s): render lines [line0, line0 + nlines) to d_out (device) */
-extern int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int16_t *d_out,
-	const int16_t *d_acc, int acc_lines, void *stream);
-/* --pixelrate: d = sample-rate context, r = raster context at the pixel rate (htv_kernels.cu) */
-extern int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0, int nlines, int16_t *d_out,
+/* the line kernel(s): render lines [line0, line0 + nlines) to d_out (device); r is NULL, or with --pixelrate the raster
+ * context at the pixel rate, d then being the sample-rate context (htv_kernels.cu) */
+extern int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, int nlines, int16_t *d_out,
 	const int16_t *d_acc, int acc_lines, void *stream);
 extern void *htv_dev_event_new_timed(htv_dev_t *d);
 extern float htv_dev_event_elapsed(void *e0, void *e1);

@@ -163,6 +163,7 @@ struct DevPlan {
 	const KFmvMod *fmv_mod;
 	const void *raster;               // k_raster or k_raster_secam where this context launches one
 	size_t raster_smem, kl_smem, ks_smem, mod_smem, fmv_smem;   // their dynamic shared memory
+	int before, after;                // lines a call rasters before its first and after its last emitted line
 	int line_threads;                 // CTA of the split kernels: a thread per 4 samples, whole warps, at least 64
 	int kl_threads;                   // CTA of the fused kernels: a warp per tile of 128 samples
 	int plane_pitch;                  // k_mod_mma: 0, the planes are the contiguous stream; else bytes per line row (htv_mma_fir.h)
@@ -214,9 +215,9 @@ struct htv_dev_t {
 	int r2_armed;
 	int side_armed;
 	int ev_pending;
-	void *d_desc_r2;                  // LineR2[cap + 2] (x 2 for the fused line kernel): the raster of PAL / NTSC / mono
+	void *d_desc_r;                   // raster descriptors [cap + before + after] (x 2 for the fused line kernel): LineS2 for
+	                                  // SECAM, LineR2 for PAL / NTSC / mono
 	void *d_desc_a2;                  // LineA2[cap + 1] (x 2 for the fused line kernel)
-	void *d_desc_s2;                  // LineS2[cap + 3]: the raster of SECAM
 	int desc_cap;                     // lines per call the descriptor buffers hold (desc_reserve)
 	int kl_ctas;                      // persistent CTAs of the fused kernels (k_line, k_sec_raster)
 	char kname[192];                  // the line kernel(s) the last render launched, with their template arguments (htv_line_kernel)
@@ -2361,6 +2362,12 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	else if(secam && !sw.split) p->path = PATH_SEC_LINE;
 	else if(!secam && !sw.split && chroma_ok && (!dp.vf_type || mma)) p->path = PATH_LINE;
 	else p->path = PATH_SPLIT;
+	// The lines a call rasters around the ones it emits, for the raster descriptors, the raster stage and the row the
+	// modulators read from: one on either side, which the video filter and the line kernels look into. SECAM's rows
+	// reach one line further back. The pixel-rate raster reaches one line further on: emitted line t is resampled line
+	// t + 1, which is made of raster lines t and t + 1.
+	p->before = secam ? 2 : 1;
+	p->after = p->path == PATH_RASTER ? 2 : 1;
 
 	p->raster_smem = sizeof(int) * 2 * (W4 + 2 * UOFF);
 	if(secam)
@@ -2481,6 +2488,15 @@ extern "C" int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, 
 	return(HTV_OK);
 }
 
+// An encoder's side streams and events, in the one list htv_dev_create creates and htv_dev_destroy destroys. ev0 and
+// ev1 time the last modulator launch (htv_dev_last_line_ms); every other event only orders work, without timing.
+struct DevSync { cudaStream_t *stream[4]; cudaEvent_t *timed[2]; cudaEvent_t *event[9]; };
+static DevSync dev_sync(htv_dev_t *d)
+{
+	return(DevSync{ { &d->side, &d->side2, &d->side3, &d->up }, { &d->ev0, &d->ev1 },
+		{ &d->ev_nic, &d->ev_up, &d->ev_chunk[0], &d->ev_chunk[1], &d->ev_in, &d->ev_kl[0], &d->ev_kl[1], &d->ev_r2, &d->ev_audio } });
+}
+
 // htv_dev_create's way out: the message, and everything allocated so far freed
 static htv_dev_t *create_fail(htv_dev_t *d, char *err, size_t errlen, const char *fmt, ...)
 {
@@ -2597,7 +2613,7 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			return(create_fail(d, err, errlen, "HTV_SEC: sub=%d is more than the %d lines of one launch", d->sec_sub, d->sub_lines));
 		d->sub_lines = d->sec_sub;
 	}
-	const size_t rows = (size_t) d->sub_lines + 3;
+	const size_t rows = (size_t) d->sub_lines + 3;       // every path's before + after is at most 3 (plan_kernels)
 	if(p.path != PATH_LINE && cudaMalloc((void **) &d->d_comp, sizeof(int16_t) * rows * W + 256) != cudaSuccess)
 		return(create_fail(d, err, errlen, "device allocation failed"));
 	if(p.path == PATH_FMV)
@@ -2680,22 +2696,13 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	}
 	if(d->alloc_failed) return(create_fail(d, err, errlen, "device allocation failed"));
 	if(!plan_attributes(p, err, errlen)) { htv_dev_destroy(d); return(NULL); }
-	cudaEventCreate(&d->ev0);
-	cudaEventCreate(&d->ev1);
-	cudaStreamCreateWithFlags(&d->side, cudaStreamNonBlocking);
-	cudaStreamCreateWithFlags(&d->side2, cudaStreamNonBlocking);
-	cudaEventCreateWithFlags(&d->ev_nic, cudaEventDisableTiming);
-	cudaStreamCreateWithFlags(&d->up, cudaStreamNonBlocking);
-	cudaEventCreateWithFlags(&d->ev_up, cudaEventDisableTiming);
-	cudaEventCreateWithFlags(&d->ev_chunk[0], cudaEventDisableTiming);
-	cudaEventCreateWithFlags(&d->ev_chunk[1], cudaEventDisableTiming);
-	cudaEventCreateWithFlags(&d->ev_in, cudaEventDisableTiming);
-	cudaEventCreateWithFlags(&d->ev_kl[0], cudaEventDisableTiming);
-	cudaEventCreateWithFlags(&d->ev_r2, cudaEventDisableTiming);
-	cudaStreamCreateWithFlags(&d->side3, cudaStreamNonBlocking);
-	cudaEventCreateWithFlags(&d->ev_kl[1], cudaEventDisableTiming);
+	const DevSync sy = dev_sync(d);
+	bool made = true;
+	for(cudaStream_t *s : sy.stream) made &= cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
+	for(cudaEvent_t *e : sy.timed) made &= cudaEventCreate(e) == cudaSuccess;
+	for(cudaEvent_t *e : sy.event) made &= cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
+	if(!made) return(create_fail(d, err, errlen, "stream or event creation failed"));
 	d->ahead = p.path == PATH_LINE && !d->sw.no_ahead;
-	cudaEventCreateWithFlags(&d->ev_audio, cudaEventDisableTiming);
 	// the table build and the memsets above ran on the default stream, which the (non-blocking)
 	// streams the encoder works on do not wait for
 	if(cudaDeviceSynchronize() != cudaSuccess)
@@ -2710,27 +2717,16 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	// the side streams may still be ahead of the caller's; nothing of this encoder is freed under running work
 	cudaDeviceSynchronize();
 	for(int i = 0; i < d->nalloc; i++) cudaFree(d->alloc[i]);
-	cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
 	if(d->h_map) cudaFreeHost(d->h_map);
 	if(d->h_ov_line) { cudaFreeHost(d->h_ov_line); cudaFreeHost(d->h_ov_meta); cudaFreeHost(d->h_ov_add); }
 	cudaFree(d->d_ov_line); cudaFree(d->d_ov_meta); cudaFree(d->d_ov_add);
 	if(d->ev_ov) cudaEventDestroy(d->ev_ov);
 	for(int i = 0; i < MAPBUFS; i++) if(d->ev_map[i]) cudaEventDestroy(d->ev_map[i]);
-	if(d->ev0) cudaEventDestroy(d->ev0);
-	if(d->ev1) cudaEventDestroy(d->ev1);
-	if(d->ev_in) cudaEventDestroy(d->ev_in);
-	if(d->ev_kl[0]) cudaEventDestroy(d->ev_kl[0]);
-	if(d->ev_r2) cudaEventDestroy(d->ev_r2);
-	if(d->side3) cudaStreamDestroy(d->side3);
-	if(d->ev_kl[1]) cudaEventDestroy(d->ev_kl[1]);
-	if(d->ev_audio) cudaEventDestroy(d->ev_audio);
-	if(d->side) cudaStreamDestroy(d->side);
-	if(d->side2) cudaStreamDestroy(d->side2);
-	if(d->ev_nic) cudaEventDestroy(d->ev_nic);
-	if(d->up) cudaStreamDestroy(d->up);
-	if(d->ev_up) cudaEventDestroy(d->ev_up);
-	if(d->ev_chunk[0]) cudaEventDestroy(d->ev_chunk[0]);
-	if(d->ev_chunk[1]) cudaEventDestroy(d->ev_chunk[1]);
+	const DevSync sy = dev_sync(d);
+	for(cudaStream_t *s : sy.stream) if(*s) cudaStreamDestroy(*s);
+	for(cudaEvent_t *e : sy.timed) if(*e) cudaEventDestroy(*e);
+	for(cudaEvent_t *e : sy.event) if(*e) cudaEventDestroy(*e);
 	free(d);
 }
 
@@ -2916,20 +2912,30 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	return(HTV_OK);
 }
 
-// The sound descriptors of lines line0 .. line0 + n - 1 into la, on every path but the fused line kernel's (which runs
-// them ahead of the caller's stream): each half on the side stream of the pre-pass chain it depends on, behind this
-// call's place in the caller's stream st; ev_audio and ev_nic mark the two halves done
-static int launch_desc_a2(htv_dev_t *d, LineA2 *la, int64_t line0, int n, cudaStream_t st)
+// The sound descriptors of lines line0 .. line0 + n - 1, each half on the side stream of the pre-pass chain it depends
+// on; ev_audio and ev_nic mark the two halves done. The fused line kernel's buffers are two, so that the next call's
+// descriptors may be written while this call's line kernel runs: with HTV_AHEAD they wait for the line kernel that last
+// read their buffer, not for the caller's stream. Every other path's wait for this call's place in the caller's stream.
+static int launch_desc_a2(htv_dev_t *d, int64_t line0, int n, cudaStream_t st, LineA2 **la)
 {
-	if(!d->side_armed)
+	*la = (LineA2 *) d->d_desc_a2 + (size_t) d->kl_buf * ((size_t) d->desc_cap + 1);
+	if(d->ahead && d->side_armed)
 	{
-		CK(cudaEventRecord(d->ev_in, st));
-		CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
+		CK(cudaStreamWaitEvent(d->side, d->ev_kl[d->kl_buf], 0));
+		CK(cudaStreamWaitEvent(d->side2, d->ev_kl[d->kl_buf], 0));
 	}
-	CK(cudaStreamWaitEvent(d->side2, d->ev_in, 0));
+	else
+	{
+		if(!d->side_armed)
+		{
+			CK(cudaEventRecord(d->ev_in, st));
+			CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
+		}
+		CK(cudaStreamWaitEvent(d->side2, d->ev_in, 0));             // ev_in: this call's place in the caller's stream (pre-pass or above)
+	}
 	const int dgrid = (n + KD_LINES * KD_WARPS - 1) / (KD_LINES * KD_WARPS);
-	k_line_desc_a2<1><<<dgrid, 32 * KD_WARPS, 0, d->side>>>(d->dp, d->dt, la, line0, n);
-	k_line_desc_a2<2><<<dgrid, 32 * KD_WARPS, 0, d->side2>>>(d->dp, d->dt, la, line0, n);
+	k_line_desc_a2<1><<<dgrid, 32 * KD_WARPS, 0, d->side>>>(d->dp, d->dt, *la, line0, n);
+	k_line_desc_a2<2><<<dgrid, 32 * KD_WARPS, 0, d->side2>>>(d->dp, d->dt, *la, line0, n);
 	CK(cudaEventRecord(d->ev_audio, d->side));
 	CK(cudaEventRecord(d->ev_nic, d->side2));
 	d->side_armed = 0;
@@ -2937,9 +2943,9 @@ static int launch_desc_a2(htv_dev_t *d, LineA2 *la, int64_t line0, int n, cudaSt
 	return(HTV_OK);
 }
 
-// The descriptor buffers of calls of up to n lines: raster descriptors (LineS2 for SECAM, else LineR2) where the context
-// rasters, sound descriptors where it modulates, two of each for the fused line kernel. Growing them first waits for
-// every stream that may still read the old ones.
+// The descriptor buffers of calls of up to n lines: raster descriptors where the context rasters, sound descriptors
+// where it modulates, two of each for the fused line kernel. Growing them first waits for every stream that may still
+// read the old ones.
 static int desc_reserve(htv_dev_t *d, int n, cudaStream_t st)
 {
 	if(n <= d->desc_cap) return(HTV_OK);
@@ -2949,18 +2955,48 @@ static int desc_reserve(htv_dev_t *d, int n, cudaStream_t st)
 	cudaStreamSynchronize(d->side);
 	cudaStreamSynchronize(d->side2);
 	cudaStreamSynchronize(d->side3);
-	cudaFree(d->d_desc_r2); cudaFree(d->d_desc_a2); cudaFree(d->d_desc_s2);
-	d->d_desc_r2 = d->d_desc_a2 = d->d_desc_s2 = NULL;
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2);
+	d->d_desc_r = d->d_desc_a2 = NULL;
 	d->desc_cap = 0;
-	if(d->dp.colour_mode == HTV_SECAM) CK(cudaMalloc(&d->d_desc_s2, sizeof(LineS2) * ((size_t) n + 3)));
-	else if(p.path != PATH_RS) CK(cudaMalloc(&d->d_desc_r2, bufs * sizeof(LineR2) * ((size_t) n + 2)));
+	static_assert(sizeof(LineS2) == sizeof(LineR2), "one raster descriptor buffer holds either");
+	if(p.path != PATH_RS) CK(cudaMalloc(&d->d_desc_r, bufs * sizeof(LineR2) * ((size_t) n + p.before + p.after)));
+	// + 1: FM video's fill line (fm_skip)
 	if(p.path != PATH_RASTER) CK(cudaMalloc(&d->d_desc_a2, bufs * sizeof(LineA2) * ((size_t) n + 1)));
 	d->desc_cap = n;
 	return(HTV_OK);
 }
 
-// The plan's split modulator over n lines (htv_dev_render_lines, htv_dev_render_lines_rs): descriptors la, the composite
-// stream as k_raster / k_resample left it for this modulator (byte planes, int32, or the int16 `comp`), output o
+// The raster descriptors of a call of n lines from line0, entry i <-> line line0 - before + i, by the context c that
+// rasters them (d, or its pixel-rate raster context); d counts the launch. Behind the frame map on side3 where
+// htv_dev_set_frame_map put it there (the overlays were staged by the host before this call), else on the caller's stream.
+static int launch_desc_r(htv_dev_t *d, htv_dev_t *c, int64_t line0, int n, cudaStream_t st, void **lr)
+{
+	const DevPlan &p = c->plan;
+	const int rows = n + p.before + p.after;
+	const bool side = c->ahead && c->r2_armed;
+	*lr = (char *) c->d_desc_r + (size_t) c->kl_buf * sizeof(LineR2) * ((size_t) c->desc_cap + p.before + p.after);
+	k_line_desc_r<<<(rows + 63) / 64, 64, 0, side ? c->side3 : st>>>(c->dp, c->dt, *lr, line0 - p.before, rows);
+	d->launches++;
+	if(side)
+	{
+		CK(cudaEventRecord(c->ev_r2, c->side3));
+		CK(cudaStreamWaitEvent(st, c->ev_r2, 0));
+		c->r2_armed = 0;
+	}
+	return(HTV_OK);
+}
+
+// The persistent grid of k_line and k_sec_raster over n rows: every CTA walks its own run of consecutive rows, at least
+// 4 (a run of k_line rasters or stages two lines more than it emits)
+static int persistent_grid(int n, int ctas, int *run)
+{
+	*run = (n + ctas - 1) / ctas;
+	if(*run < 4) *run = 4;
+	return((n + *run - 1) / *run);
+}
+
+// The plan's split modulator over n lines: descriptors la, the composite stream as k_raster / k_resample left it for
+// this modulator (byte planes, int32, or the int16 `comp`), output o
 static void launch_mod(const htv_dev_t *d, int n, const LineA2 *la, const int16_t *comp, int16_t *o, const int16_t *acc,
 	int acc_rows, cudaStream_t st)
 {
@@ -2972,214 +3008,72 @@ static void launch_mod(const htv_dev_t *d, int n, const LineA2 *la, const int16_
 	else m.mod<<<n, p.line_threads, p.mod_smem, st>>>(d->dp, d->dt, la, comp, o, acc, acc_rows);
 }
 
-extern "C" int htv_dev_render_lines(htv_dev_t *d, int64_t line0, int nlines, int16_t *d_out,
-	const int16_t *d_acc, int acc_lines, void *stream)
+// The SECAM chrominance chain (htv_secam.cuh) over a sub-batch of n lines, whose raster rows start at ls (rows 0 .. n + 2
+// <-> lines first - 2 .. first + n): pass 0 over every line, the predictor, then refinement passes until no line's
+// outgoing state changes - at that fixed point every line was computed from its true predecessor state = the
+// sequential result. The loop needs the change count on the host, so SECAM launches synchronise.
+static int sec_chain(htv_dev_t *d, const LineS2 *ls, int n, cudaStream_t st)
 {
-	DevGuard guard(d->device);
-	cudaStream_t st = (cudaStream_t) stream;
-	const DevPlan &p = d->plan;
-	if(nlines <= 0) return(HTV_OK);
-	// FM video with a pre-emphasis filter: the modulator also integrates the pipeline's fill line
-	const int fm_skip = d->dp.have_fmv && d->dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
-	if(desc_reserve(d, nlines, st) != HTV_OK) return(HTV_ERROR);
-	const bool secam = d->dp.colour_mode == HTV_SECAM;
-	if(p.path == PATH_LINE)
+	const int nch = n + 2, nb = (nch + 31) / 32;     // the chain's rows: 0 .. n + 1, lines first - 2 .. first + n - 1
+	cudaEvent_t dbg0 = NULL, dbg1 = NULL;
+	const bool dbg = d->sw.debug;
+	if(dbg) { cudaEventCreate(&dbg0); cudaEventCreate(&dbg1); cudaEventRecord(dbg0, st); }
+	int pass = 0, changed = 1, repredict = d->sec_repredict;
+	htv_secam_chain_t &cs = d->sec_stats;
+	cs.launches++;
+	for(; pass <= d->sec_passes && changed; pass++)
 	{
-		// one persistent launch for the whole call: every CTA walks its own run of consecutive lines
-		const htv_dparams_t &dp = d->dp;
-		LineR2 *lr2 = (LineR2 *) d->d_desc_r2 + (size_t) d->kl_buf * ((size_t) d->desc_cap + 2);
-		if(d->ahead && d->r2_armed)
+		int fl[4];
+		cudaMemsetAsync(d->sec.flags, 0, sizeof(int) * 4, st);
+		if(pass == 0)
 		{
-			// behind the frame map on side3 (htv_dev_set_frame_map); overlays were staged by the host before this call
-			k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, d->side3>>>(dp, d->dt, lr2, line0 - 1, nlines + 2);
-			CK(cudaEventRecord(d->ev_r2, d->side3));
-			CK(cudaStreamWaitEvent(st, d->ev_r2, 0));
-			d->r2_armed = 0;
-		}
-		else k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, st>>>(dp, d->dt, lr2, line0 - 1, nlines + 2);
-		if(!d->side_armed)
-		{
-			CK(cudaEventRecord(d->ev_in, st));
-			CK(cudaStreamWaitEvent(d->side, d->ev_in, 0));
-		}
-		// sound descriptors: two buffers, so that the next call's may be written while this call's line kernel runs
-		const int buf = d->kl_buf;
-		d->kl_buf ^= 1;
-		LineA2 *la2 = (LineA2 *) d->d_desc_a2 + (size_t) buf * ((size_t) d->desc_cap + 1);
-		// the two halves of the sound descriptors, each on the side stream of the pre-pass chain it depends on
-		const int dgrid = (nlines + KD_LINES * KD_WARPS - 1) / (KD_LINES * KD_WARPS);
-		if(d->ahead && d->side_armed)
-		{
-			CK(cudaStreamWaitEvent(d->side, d->ev_kl[buf], 0));
-			CK(cudaStreamWaitEvent(d->side2, d->ev_kl[buf], 0));
-		}
-		else CK(cudaStreamWaitEvent(d->side2, d->ev_in, 0));             // ev_in: this call's place in the caller's stream (pre-pass or above)
-		k_line_desc_a2<1><<<dgrid, 32 * KD_WARPS, 0, d->side>>>(dp, d->dt, la2, line0, nlines);
-		k_line_desc_a2<2><<<dgrid, 32 * KD_WARPS, 0, d->side2>>>(dp, d->dt, la2, line0, nlines);
-		CK(cudaEventRecord(d->ev_audio, d->side));
-		CK(cudaEventRecord(d->ev_nic, d->side2));
-		d->side_armed = 0;
-		CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
-		CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
-		// runs of at least 4 lines (every run rasters two lines more than it emits)
-		int run = (nlines + d->kl_ctas - 1) / d->kl_ctas;
-		if(run < 4) run = 4;
-		const int grid = (nlines + run - 1) / run;
-		if(d->timing) cudaEventRecord(d->ev0, st);
-		strcpy(d->kname, p.kname);
-		p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, lr2, la2, nlines, run, d_out, d_acc, d_acc ? acc_lines : 0, NULL);
-		CK(cudaEventRecord(d->ev_kl[buf], st));
-		d->launches += 4;
-		d->last_mod_lines = nlines;
-		if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
-		CK(cudaEventRecord(d->ev_chunk[d->chunk_i & 1], st));
-		d->chunk_i++;
-		CK(cudaGetLastError());
-		return(HTV_OK);
-	}
-	// raster descriptors: SECAM's ls0[i] <-> line line0 - 2 + i (its rows reach one line further back), lr0[i] <-> line line0 - 1 + i
-	const LineS2 *ls0 = (const LineS2 *) d->d_desc_s2;
-	const LineR2 *lr0 = (const LineR2 *) d->d_desc_r2;
-	if(secam) k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, d->d_desc_s2, line0 - 2, nlines + 3);
-	else k_line_desc_r<<<(nlines + 2 + 63) / 64, 64, 0, st>>>(d->dp, d->dt, d->d_desc_r2, line0 - 1, nlines + 2);
-	d->launches++;
-	// la2[i] <-> line line0 - fm_skip + i
-	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
-	if(launch_desc_a2(d, la2, line0 - fm_skip, nlines + fm_skip, st) != HTV_OK) return(HTV_ERROR);
-	bool joined = false;
-	for(int done = 0; done < nlines; done += d->sub_lines)
-	{
-		const int n = nlines - done < d->sub_lines ? nlines - done : d->sub_lines;
-		const bool last = done + n >= nlines;
-		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * d->dp.W * htv_st_bytes(d->dp.sample_type, d->dp.complex_out));
-		const int16_t *cstream = d->d_comp;
-		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
-		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * d->dp.W * (d->dp.complex_out ? 2 : 1) : NULL;
-		const int acc_rows = acc ? acc_lines - done : 0;
-		if(secam)
-		{
-			// rows 0 .. n+2 <-> lines first-2 .. first+n; the chain covers rows 0 .. n+1
-			const LineS2 *ls = ls0 + done;
-			if(p.ks)
-			{
-				// rows 0 .. n+2 in runs of rows per persistent CTA
-				const int nr = n + 3;
-				int run = (nr + d->kl_ctas - 1) / d->kl_ctas;
-				if(run < 4) run = 4;
-				const int grid = (nr + run - 1) / run;
-				p.ks->fn<<<grid, p.kl_threads, p.ks_smem, st>>>(d->dp, d->dt, ls, nr, run, d->d_comp, d->sec);
-				d->launches++;
-			}
-			else k_raster_secam<<<n + 3, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, ls, d->d_comp, d->sec);
-			// the chain (htv_secam.cuh): pass 0 over every line, the predictor, then refinement passes until no line's
-			// outgoing state changes - at that fixed point every line was computed from its true predecessor state =
-			// the sequential result. The loop needs the change count on the host, so SECAM launches synchronise.
-			const int nch = n + 2, nb = (nch + 31) / 32;
-			cudaEvent_t dbg0 = NULL, dbg1 = NULL;
-			const bool dbg = d->sw.debug;
-			if(dbg) { cudaEventCreate(&dbg0); cudaEventCreate(&dbg1); cudaEventRecord(dbg0, st); }
-			int pass = 0, changed = 1, repredict = d->sec_repredict;
-			htv_secam_chain_t &cs = d->sec_stats;
-			cs.launches++;
-			for(; pass <= d->sec_passes && changed; pass++)
-			{
-				int fl[4];
-				cudaMemsetAsync(d->sec.flags, 0, sizeof(int) * 4, st);
-				if(pass == 0)
-				{
-					k_sec_pass0<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch);
-					// propose the states pass 1 starts from (see k_sec_predict); st[0] takes them over
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
-					cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
-					d->launches += 2;
-					continue;
-				}
-				k_sec_refine<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, pass);
-				k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
-				k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
-				d->launches += 3;
-				CK(cudaMemcpyAsync(fl, d->sec.flags, sizeof(fl), cudaMemcpyDeviceToHost, st));
-				CK(cudaStreamSynchronize(st));
-				changed = fl[0];
-				// what the chain did, from the counts this pass copies back anyway
-				cs.passes++;
-				cs.recomputed += fl[2];
-				if(fl[3] > d->sec_many) cs.listed_thread += fl[3]; else cs.listed_warp += fl[3];
-				if(fl[3] > cs.list_max) cs.list_max = fl[3];
-				if(dbg)
-				{
-					float ms = 0;
-					cudaEventRecord(dbg1, st); cudaEventSynchronize(dbg1); cudaEventElapsedTime(&ms, dbg0, dbg1);
-					fprintf(stderr, "secam pass %d: recomputed %d (FM in full: %d), output changed %d, cumulative %.3f ms\n", pass, fl[2], fl[3], fl[0], ms);
-				}
-				if(changed && fl[3] > d->sec_repredict_min && repredict > 0)
-				{
-					// many lines had their FM recurrence re-run: their A, B moved, and plain iteration would carry that down
-					// the lines at 3x per pass - propose again from the new checkpoints (the pass's outputs go to st[0] first)
-					repredict--;
-					if(pass & 1) cs.repredict_odd++; else cs.repredict_even++;
-					if(pass & 1) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
-					k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
-					if(!(pass & 1)) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
-					d->launches++;
-				}
-			}
-			if(pass - 1 > cs.passes_max) cs.passes_max = pass - 1;
-			if(changed)
-			{
-				fprintf(stderr, "hacktv_b200: SECAM cross-line state did not converge in %d passes\n", d->sec_passes);
-				return(HTV_ERROR);
-			}
-			if((pass - 1) & 1) cs.final_odd++; else cs.final_even++;
-			k_sec_carry<<<1, 32, 0, st>>>(ls, d->sec, n - 1, pass - 1);
-			k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, ls, d->sec, d->d_comp, nch);
+			k_sec_pass0<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch);
+			// propose the states pass 1 starts from (see k_sec_predict); st[0] takes them over
+			k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
+			cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 			d->launches += 2;
-			if(d->dt.ov_n > 0)
-			{
-				k_overlay_secam<<<n + 3, 256, 0, st>>>(d->dp, d->dt, line0 + done - 2, d->d_comp);
-				d->launches++;
-			}
-			cstream = d->d_comp + d->dp.W;          // k_mod's line b sits at row b + 2
+			continue;
 		}
-		else
+		k_sec_refine<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, pass);
+		k_sec_fm_list<<<512, 32 * SEC_LIST_WARPS, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
+		k_sec_fm_list_t<<<nb, 32, 0, st>>>(d->dp, d->dt, ls, d->sec, pass, d->sec_many);
+		d->launches += 3;
+		CK(cudaMemcpyAsync(fl, d->sec.flags, sizeof(fl), cudaMemcpyDeviceToHost, st));
+		CK(cudaStreamSynchronize(st));
+		changed = fl[0];
+		// what the chain did, from the counts this pass copies back anyway
+		cs.passes++;
+		cs.recomputed += fl[2];
+		if(fl[3] > d->sec_many) cs.listed_thread += fl[3]; else cs.listed_warp += fl[3];
+		if(fl[3] > cs.list_max) cs.list_max = fl[3];
+		if(dbg)
 		{
-			// raster lines done-1 .. done+n (descriptor index = line - (line0 - 1))
-			k_raster<<<n + 2, p.line_threads, p.raster_smem, st>>>(d->dp, d->dt, lr0 + done, d->d_comp, d->d_comp32, d->d_planes, d->plane_stride, p.plane_pitch);
+			float ms = 0;
+			cudaEventRecord(dbg1, st); cudaEventSynchronize(dbg1); cudaEventElapsedTime(&ms, dbg0, dbg1);
+			fprintf(stderr, "secam pass %d: recomputed %d (FM in full: %d), output changed %d, cumulative %.3f ms\n", pass, fl[2], fl[3], fl[0], ms);
+		}
+		if(changed && fl[3] > d->sec_repredict_min && repredict > 0)
+		{
+			// many lines had their FM recurrence re-run: their A, B moved, and plain iteration would carry that down
+			// the lines at 3x per pass - propose again from the new checkpoints (the pass's outputs go to st[0] first)
+			repredict--;
+			if(pass & 1) cs.repredict_odd++; else cs.repredict_even++;
+			if(pass & 1) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
+			k_sec_predict<<<(nch + SEC_PRED_T - SEC_PRED_HALO - 1) / (SEC_PRED_T - SEC_PRED_HALO), SEC_PRED_T, 0, st>>>(d->dp, d->dt, ls, d->sec, nch, d->sec_pred);
+			if(!(pass & 1)) cudaMemcpyAsync(d->sec.st[0], d->sec.st[1], sizeof(SecState) * nch, cudaMemcpyDeviceToDevice, st);
 			d->launches++;
 		}
-		if(!joined)
-		{
-			CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
-			CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
-			joined = true;
-		}
-		if(d->timing && last) cudaEventRecord(d->ev0, st);
-		if(p.path == PATH_FMV)
-		{
-			const int pre = fm_skip && done == 0 ? 1 : 0, rows = n + pre;
-			const LineA2 *lap = la2 + done + fm_skip - pre;
-			p.fmv_base->fn<<<rows, p.line_threads, p.fmv_smem, st>>>(d->dp, d->dt, lap, cstream, pre);
-			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, rows);
-			p.fmv_mod->fn<<<rows, p.line_threads, 0, st>>>(d->dp, d->dt, lap, o, acc, acc_rows, -pre);
-			d->launches += 2;
-		}
-		else if(p.path == PATH_SEC_LINE)
-		{
-			// runs of at least 4 lines (every run stages two lines more than it emits)
-			int run = (n + d->kl_ctas - 1) / d->kl_ctas;
-			if(run < 4) run = 4;
-			const int grid = (n + run - 1) / run;
-			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(d->dp, d->dt, NULL, la2 + done, n, run, o, acc, acc_rows, d->d_comp);
-		}
-		else launch_mod(d, n, la2 + done, cstream, o, acc, acc_rows, st);
-		strcpy(d->kname, p.kname);
-		d->launches++;
-		if(last) d->last_mod_lines = n;
 	}
-	if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
-	CK(cudaEventRecord(d->ev_chunk[d->chunk_i & 1], st));
-	d->chunk_i++;
-	CK(cudaGetLastError());
+	if(pass - 1 > cs.passes_max) cs.passes_max = pass - 1;
+	if(changed)
+	{
+		fprintf(stderr, "hacktv_b200: SECAM cross-line state did not converge in %d passes\n", d->sec_passes);
+		return(HTV_ERROR);
+	}
+	if((pass - 1) & 1) cs.final_odd++; else cs.final_even++;
+	k_sec_carry<<<1, 32, 0, st>>>(ls, d->sec, n - 1, pass - 1);
+	k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, ls, d->sec, d->d_comp, nch);
+	d->launches += 2;
 	return(HTV_OK);
 }
 
@@ -3222,57 +3116,118 @@ k_resample(const int16_t *comp, int Wp, int Ws, int I, int D, int A, const int16
 	}
 }
 
-// d: the sample-rate context (sound carriers, video filter, output); r: the raster context built
-// from tables at the pixel rate (pictures, frame map and VBI overlays are uploaded to it).
-extern "C" int htv_dev_render_lines_rs(htv_dev_t *d, htv_dev_t *r, int64_t line0, int nlines, int16_t *d_out,
+// Lines line0 .. line0 + nlines - 1 into d_out. d is the encoder; r is NULL, or with --pixelrate the raster context built
+// from tables at the pixel rate (pictures, frame map and VBI overlays are uploaded to it), whose lines k_resample brings
+// to d's rate. The raster and sound descriptors of the whole call come first, then each sub-batch runs a raster stage
+// into the composite scratch and a modulator stage from it. The fused line kernel rasters its own lines in one
+// persistent launch over the whole call: its one sub-batch has no raster stage.
+extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, int nlines, int16_t *d_out,
 	const int16_t *d_acc, int acc_lines, void *stream)
 {
 	DevGuard guard(d->device);
 	cudaStream_t st = (cudaStream_t) stream;
-	if(nlines <= 0) return(HTV_OK);
 	const DevPlan &p = d->plan;
-	if(p.path != PATH_RS || r->plan.path != PATH_RASTER || p.plane_pitch || (d->dp.W & 3)) return(HTV_ERROR);
-	if(desc_reserve(d, nlines, st) != HTV_OK || desc_reserve(r, nlines + 1, st) != HTV_OK) return(HTV_ERROR);
-	// raster descriptors lr0[i] <-> line line0 - 1 + i for lines line0 - 1 .. line0 + nlines + 1 (one line more than
-	// without a resampler: the emitted line t is resampled line t + 1 and the video filter looks into t + 2)
-	const LineR2 *lr0 = (const LineR2 *) r->d_desc_r2;
-	LineA2 *la2 = (LineA2 *) d->d_desc_a2;
-	k_line_desc_r<<<(nlines + 3 + 63) / 64, 64, 0, st>>>(r->dp, r->dt, r->d_desc_r2, line0 - 1, nlines + 3);
-	d->launches++;
-	if(launch_desc_a2(d, la2, line0, nlines, st) != HTV_OK) return(HTV_ERROR);
-	bool joined = false;
-	const int Ws = d->dp.W, Wp = r->dp.W;
-	int sub = d->sub_lines < r->sub_lines ? d->sub_lines : r->sub_lines;
-	for(int done = 0; done < nlines; done += sub)
+	const htv_dparams_t &dp = d->dp;
+	if(nlines <= 0) return(HTV_OK);
+	if((p.path == PATH_RS) != (r != NULL) || (r && (r->plan.path != PATH_RASTER || p.plane_pitch || (dp.W & 3)))) return(HTV_ERROR);
+	const bool secam = dp.colour_mode == HTV_SECAM;
+	// FM video with a pre-emphasis filter: the modulator also integrates the pipeline's fill line
+	const int fm_skip = dp.have_fmv && dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
+	if(desc_reserve(d, nlines, st) != HTV_OK || (r && desc_reserve(r, nlines, st) != HTV_OK)) return(HTV_ERROR);
+	void *desc_r;                                   // entry i <-> line line0 - before + i
+	LineA2 *la2;                                    // la2[i] <-> line line0 - fm_skip + i
+	if(launch_desc_r(d, r ? r : d, line0, nlines, st, &desc_r) != HTV_OK ||
+		launch_desc_a2(d, line0 - fm_skip, nlines + fm_skip, st, &la2) != HTV_OK) return(HTV_ERROR);
+	int sub = p.path == PATH_LINE ? nlines : d->sub_lines;
+	if(r && r->sub_lines < sub) sub = r->sub_lines;
+	// where the split and FM-video modulators read the composite scratch: line b of the sub-batch at row b + 1
+	const int16_t *comp = d->d_comp + (size_t) (p.before - 1) * dp.W;
+	int n = 0;
+	for(int done = 0; done < nlines; done += n)
 	{
-		const int n = nlines - done < sub ? nlines - done : sub;
-		const bool last = done + n >= nlines;
-		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * Ws * htv_st_bytes(d->dp.sample_type, d->dp.complex_out));
-		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * Ws * (d->dp.complex_out ? 2 : 1) : NULL;
+		n = nlines - done < sub ? nlines - done : sub;
+		const int rows = n + p.before + p.after;
+		int16_t *o = (int16_t *) ((char *) d_out + (size_t) done * dp.W * htv_st_bytes(dp.sample_type, dp.complex_out));
+		// the stream to sum into (channel combiner): its first acc_lines lines, laid out like d_out
+		const int16_t *acc = d_acc && acc_lines > done ? d_acc + (size_t) done * dp.W * (dp.complex_out ? 2 : 1) : NULL;
 		const int acc_rows = acc ? acc_lines - done : 0;
-		// raster lines line0 + done - 1 .. line0 + done + n + 1 -> rows 0 .. n + 2 of the raster context's int16 stream
-		k_raster<<<n + 3, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt, lr0 + done, r->d_comp, NULL, NULL, 0, 0);
-		// resampled lines line0 + done .. line0 + done + n + 1 -> rows 0 .. n + 1 of this context's scratch
-		k_resample<<<n + 2, p.line_threads, 0, st>>>(r->d_comp, Wp, Ws, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
-			d->d_planes, d->plane_stride, d->d_comp32, d->d_comp);
-		d->launches += 2;
-		if(!joined)
+		// raster stage
+		if(r)
+		{
+			// the raster at the pixel rate into r's int16 stream, then the rows this context's modulator reads
+			k_raster<<<n + r->plan.before + r->plan.after, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt,
+				(const LineR2 *) desc_r + done, r->d_comp, NULL, NULL, 0, 0);
+			k_resample<<<rows, p.line_threads, 0, st>>>(r->d_comp, r->dp.W, dp.W, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
+				d->d_planes, d->plane_stride, d->d_comp32, d->d_comp);
+			d->launches += 2;
+		}
+		else if(secam)
+		{
+			const LineS2 *ls = (const LineS2 *) desc_r + done;
+			if(p.ks)
+			{
+				int run;
+				const int grid = persistent_grid(rows, d->kl_ctas, &run);
+				p.ks->fn<<<grid, p.kl_threads, p.ks_smem, st>>>(dp, d->dt, ls, rows, run, d->d_comp, d->sec);
+				d->launches++;
+			}
+			else k_raster_secam<<<rows, p.line_threads, p.raster_smem, st>>>(dp, d->dt, ls, d->d_comp, d->sec);
+			if(sec_chain(d, ls, n, st) != HTV_OK) return(HTV_ERROR);
+			if(d->dt.ov_n > 0)
+			{
+				k_overlay_secam<<<rows, 256, 0, st>>>(dp, d->dt, line0 + done - p.before, d->d_comp);
+				d->launches++;
+			}
+		}
+		else if(p.path != PATH_LINE)
+		{
+			k_raster<<<rows, p.line_threads, p.raster_smem, st>>>(dp, d->dt, (const LineR2 *) desc_r + done, d->d_comp, d->d_comp32,
+				d->d_planes, d->plane_stride, p.plane_pitch);
+			d->launches++;
+		}
+		if(done == 0)
 		{
 			CK(cudaStreamWaitEvent(st, d->ev_audio, 0));
 			CK(cudaStreamWaitEvent(st, d->ev_nic, 0));
-			joined = true;
 		}
-		if(d->timing && last) cudaEventRecord(d->ev0, st);
-		launch_mod(d, n, la2 + done, d->d_comp, o, acc, acc_rows, st);
+		// modulator stage
+		if(d->timing && done + n >= nlines) cudaEventRecord(d->ev0, st);
+		if(p.kl)
+		{
+			// k_line from its own raster, or k_line<SRC> from the SECAM raster stage's rows
+			int run;
+			const int grid = persistent_grid(n, d->kl_ctas, &run);
+			const bool line = p.path == PATH_LINE;
+			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, line ? (const LineR2 *) desc_r : NULL, la2 + done, n, run,
+				o, acc, acc_rows, line ? NULL : d->d_comp);
+			if(line)
+			{
+				// this call's descriptor buffers are free again once ev_kl has passed; the next call takes the other two
+				CK(cudaEventRecord(d->ev_kl[d->kl_buf], st));
+				d->kl_buf ^= 1;
+			}
+		}
+		else if(p.path == PATH_FMV)
+		{
+			const int pre = fm_skip && done == 0 ? 1 : 0, frows = n + pre;
+			const LineA2 *lap = la2 + done + fm_skip - pre;
+			p.fmv_base->fn<<<frows, p.line_threads, p.fmv_smem, st>>>(dp, d->dt, lap, comp, pre);
+			k_fmv_scan<<<1, 1024, 0, st>>>(d->dt, frows);
+			p.fmv_mod->fn<<<frows, p.line_threads, 0, st>>>(dp, d->dt, lap, o, acc, acc_rows, -pre);
+			d->launches += 2;
+		}
+		else launch_mod(d, n, la2 + done, comp, o, acc, acc_rows, st);
 		d->launches++;
-		strcpy(d->kname, p.kname);
-		if(last) d->last_mod_lines = n;
 	}
 	if(d->timing) { cudaEventRecord(d->ev1, st); d->ev_pending = 1; }
-	CK(cudaEventRecord(d->ev_chunk[d->chunk_i & 1], st));
-	d->chunk_i++;
-	CK(cudaEventRecord(r->ev_chunk[r->chunk_i & 1], st));
-	r->chunk_i++;
+	d->last_mod_lines = n;
+	strcpy(d->kname, p.kname);
+	htv_dev_t *const ctx[] = { d, r };
+	for(htv_dev_t *c : ctx) if(c)
+	{
+		CK(cudaEventRecord(c->ev_chunk[c->chunk_i & 1], st));
+		c->chunk_i++;
+	}
 	CK(cudaGetLastError());
 	return(HTV_OK);
 }

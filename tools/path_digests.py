@@ -1,9 +1,10 @@
-"""Byte identity of the split, FM-video and --pixelrate paths across builds: sha256 of each case's output.
+"""Byte identity of the device paths across builds: sha256 of each case's output, with its launch count.
 
 Every case renders a fixed number of lines of the test source in uneven calls (1, 2, 23, 300, 625, 2000, ... lines),
 so that sub-batch, descriptor-buffer and stream-start edges fall at different places, and prints one JSON line:
-{"case", "line_kernel", "lines", "sha256"}. Run it against two builds of the library (HTV_LIB=<other .so>) and
-compare the lines: every digest must match where the two builds are meant to compute the same stream.
+{"case", "line_kernel", "kernel_launches", "secam_chain", "lines", "sha256"}. Run it against two builds of the library
+(HTV_LIB=<other .so>) and compare the lines: where the two builds are meant to compute the same stream in the same
+launches, every line must match - the digest, the launch count and the SECAM chain's counters.
 
 --time adds, for the timed cases, the device-resident ms of one 64-frame htv_render call (CUDA events around the
 call on its stream, median of --reps calls after --warmup), with the card's name and power limit.
@@ -47,6 +48,8 @@ CASES = [
     ("pal-fm_20M_filter_float", "pal-fm", dict(vfilter=True), 20_000_000, 0, {}, "float", 900),
     ("i_16M_filter_split_long", "i", dict(vfilter=True), 16_000_000, 0, SPLIT, "int16", 20_500),
     ("i_16M_filter_default", "i", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
+    # the fused line kernel's sound pre-pass and descriptors in the caller's stream order
+    ("i_16M_filter_default_no_ahead", "i", dict(vfilter=True), 16_000_000, 0, dict(HTV_AHEAD="0"), "int16", 1400),
     ("l_16M_filter_default", "l", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
     # SECAM: k_raster_secam + chain + k_line<SRC>; the same behind the split modulator; at 13.5 Msps the chain's
     # work-list kernels run; baseband (no video filter)
@@ -58,12 +61,17 @@ CASES = [
     ("i_16M_from_14M_filter", "i", dict(vfilter=True), 16_000_000, 14_000_000, {}, "int16", 1400),
 ]
 
-# split render_add: the second channel added into the first one's stream
-ADD_CASE = ("i_16M_filter_split_render_add", "i", dict(vfilter=True, offset=-3_000_000, level=0.5),
-            dict(vfilter=True, offset=2_500_000, level=0.5), 16_000_000, SPLIT, 1400)
+# render_add: the second channel added into the first one's stream, split and --pixelrate
+ADD_CASES = [
+    ("i_16M_filter_split_render_add", "i", dict(vfilter=True, offset=-3_000_000, level=0.5),
+     dict(vfilter=True, offset=2_500_000, level=0.5), 16_000_000, 0, SPLIT, 1400),
+    ("i_16M_from_13M5_filter_render_add", "i", dict(vfilter=True, offset=-3_000_000, level=0.5),
+     dict(vfilter=True, offset=2_500_000, level=0.5), 16_000_000, 13_500_000, {}, 1400),
+]
 
 TIMED = ["i_16M_filter_split_mma", "i_16M_filter_split_tma", "pal-fm_20M", "pal-fm_20M_filter",
-         "i_16M_from_13M5_filter", "i_16M_from_13M5", "l_16M_filter_split", "i_10M_split", "l_16M_filter_default"]
+         "i_16M_from_13M5_filter", "i_16M_from_13M5", "l_16M_filter_split", "i_10M_split", "l_16M_filter_default",
+         "i_16M_filter_default", "i_16M_filter_default_no_ahead"]
 
 
 def card():
@@ -76,7 +84,7 @@ def card():
 
 
 def encoder(mode, kw, rate, prate, env, sample_type):
-    for k in ("HTV_PATH", "HTV_FIR"):
+    for k in ("HTV_PATH", "HTV_FIR", "HTV_AHEAD"):
         os.environ.pop(k, None)
     os.environ.update(env)                          # read once per encoder, when it is created
     enc = H.Encoder(H.mode_config(mode, **kw), rate, prate)
@@ -100,15 +108,16 @@ def digest(name, mode, kw, rate, prate, env, sample_type, lines):
     h = hashlib.sha256()
     for n in pieces(lines):
         h.update(np.ascontiguousarray(enc.render_host(n)).tobytes())
-    r = {"case": name, "line_kernel": enc.line_kernel, "lines": lines, "sha256": h.hexdigest()}
+    r = {"case": name, "line_kernel": enc.line_kernel, "kernel_launches": enc.kernel_launches,
+         "secam_chain": enc.secam_chain, "lines": lines, "sha256": h.hexdigest()}
     enc.close()
     return r
 
 
-def digest_add(name, mode, kw_a, kw_b, rate, env, lines):
+def digest_add(name, mode, kw_a, kw_b, rate, prate, env, lines):
     import torch
-    a = encoder(mode, kw_a, rate, 0, env, "int16")
-    b = encoder(mode, kw_b, rate, 0, env, "int16")
+    a = encoder(mode, kw_a, rate, prate, env, "int16")
+    b = encoder(mode, kw_b, rate, prate, env, "int16")
     per_line = a.width * (2 if a.complex else 1)
     buf = torch.zeros(lines * per_line, dtype=torch.int16, device="cuda")
     st = torch.cuda.current_stream().cuda_stream
@@ -119,7 +128,8 @@ def digest_add(name, mode, kw_a, kw_b, rate, env, lines):
         b.render_add(n, p, st)
         done += n
     torch.cuda.synchronize()
-    r = {"case": name, "line_kernel": b.line_kernel, "lines": lines,
+    r = {"case": name, "line_kernel": b.line_kernel, "kernel_launches": [a.kernel_launches, b.kernel_launches],
+         "secam_chain": [a.secam_chain, b.secam_chain], "lines": lines,
          "sha256": hashlib.sha256(buf.cpu().numpy().tobytes()).hexdigest()}
     a.close()
     b.close()
@@ -159,8 +169,9 @@ def main():
     for c in CASES:
         if want(c[0]):
             print(json.dumps(digest(*c)), flush=True)
-    if want(ADD_CASE[0]):
-        print(json.dumps(digest_add(*ADD_CASE)), flush=True)
+    for c in ADD_CASES:
+        if want(c[0]):
+            print(json.dumps(digest_add(*c)), flush=True)
     if a.time:
         for c in CASES:
             if c[0] in TIMED and want(c[0]):
