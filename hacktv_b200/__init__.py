@@ -269,6 +269,11 @@ class Encoder:
         self.active_lines = self._L.htv_active_lines(h)
         self.complex = bool(self._L.htv_is_complex(h))
         self.bytes_per_sample = self._L.htv_bytes_per_sample(h)
+        # the raster's line width, which VBI overlays are drawn at: with --pixelrate the pixel rate's
+        t = Tables(self.conf, sample_rate, pixel_rate)
+        g = t.get("rs_geometry")
+        t.close()
+        self.raster_width = self.width if g is None else int(g[3])
         self._sample_type = "int16"
         self.sample_rate = sample_rate
         self._keep = []
@@ -378,7 +383,7 @@ class Encoder:
             arr[i].replace_from, arr[i].replace_to, arr[i].replace_value = rep
             if add is not None:
                 add = np.ascontiguousarray(add, dtype=np.int16)
-                assert add.size == self.width
+                assert add.size == self.raster_width
                 self._keep.append(add)
                 arr[i].add = add.ctypes.data
         n = len(lines)

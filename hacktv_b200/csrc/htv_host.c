@@ -552,7 +552,9 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 	}
 	if(s->vbi_read || s->nov)
 	{
-		r = send_overlays(s, L0 + n);
+		/* the raster reaches two lines past the last one emitted: the video filter looks one line ahead, and with
+		 * --pixelrate emitted line t is resampled from raster lines t and t + 1 */
+		r = send_overlays(s, L0 + n + 2);
 		if(r != HTV_OK) UP_FAIL(r);
 	}
 #undef UP_FAIL

@@ -1108,6 +1108,72 @@ __device__ __forceinline__ void chroma_fir4(const htv_dparams_t &dp, const int *
 	}
 }
 
+// A thread's composite values x0 .. x0 + 3 (x0 < W) of launch row blockIdx.x, stored where the split modulators read
+// them: the byte planes when `planes` is set (pitched when plane_pitch is), else the int32 stream when `comp32` is, else
+// the int16 stream. k_raster and k_resample both store through here, so every layout a plan can select is written.
+__device__ __forceinline__ void store_line4(const int (&val)[SPT], int x0, int W, int16_t *comp, int *comp32,
+	uint8_t *planes, size_t plane_stride, int plane_pitch)
+{
+	if(planes && plane_pitch)
+	{
+		// pitched byte planes (htv_mma_fir.h): one self-contained row per line, the first / last
+		// MF_LEAD samples repeated in the halo of the previous / next row of this launch
+		uint8_t *rowp = planes + (size_t) blockIdx.x * plane_pitch;
+		if(x0 + SPT <= W)
+		{
+			*reinterpret_cast<unsigned *>(rowp + MF_LEAD + x0) = ((val[0] >> 8) & 0xFF) | (((val[1] >> 8) & 0xFF) << 8) |
+				(((val[2] >> 8) & 0xFF) << 16) | ((unsigned) (val[3] >> 8) << 24);
+			*reinterpret_cast<unsigned *>(rowp + plane_stride + MF_LEAD + x0) = (val[0] & 0xFF) | ((val[1] & 0xFF) << 8) |
+				((val[2] & 0xFF) << 16) | ((unsigned) val[3] << 24);
+		}
+		const bool head = x0 < MF_LEAD && blockIdx.x > 0, tail = x0 + SPT > W - MF_LEAD && blockIdx.x + 1 < gridDim.x;
+		if(head || tail || x0 + SPT > W)
+		{
+			#pragma unroll
+			for(int k = 0; k < SPT; k++)
+			{
+				const int x = x0 + k;
+				if(x >= W) break;
+				const uint8_t hi = (uint8_t) ((val[k] >> 8) & 0xFF), lo = (uint8_t) (val[k] & 0xFF);
+				if(x0 + SPT > W) { rowp[MF_LEAD + x] = hi; rowp[plane_stride + MF_LEAD + x] = lo; }
+				if(head && x < MF_LEAD) { uint8_t *q = rowp - plane_pitch + MF_LEAD + W + x; q[0] = hi; q[plane_stride] = lo; }
+				if(tail && x >= W - MF_LEAD) { uint8_t *q = rowp + plane_pitch + (x - (W - MF_LEAD)); q[0] = hi; q[plane_stride] = lo; }
+			}
+		}
+		return;
+	}
+	if(planes)
+	{
+		// high / low byte planes for the tensor-core video filter (k_mod_mma): v = 256 hi + lo
+		uint8_t *p = planes + (size_t) blockIdx.x * W + x0;
+		*reinterpret_cast<unsigned *>(p) = ((val[0] >> 8) & 0xFF) | (((val[1] >> 8) & 0xFF) << 8) |
+			(((val[2] >> 8) & 0xFF) << 16) | ((unsigned) (val[3] >> 8) << 24);
+		*reinterpret_cast<unsigned *>(p + plane_stride) = (val[0] & 0xFF) | ((val[1] & 0xFF) << 8) |
+			((val[2] & 0xFF) << 16) | ((unsigned) val[3] << 24);
+		return;
+	}
+	if(comp32)
+	{
+		// int32 stream for the TMA-fed modulator (values are int16-wrapped as the reference's buffer is)
+		*reinterpret_cast<int4 *>(comp32 + (size_t) blockIdx.x * W + x0) =
+			make_int4(wrap16i(val[0]), wrap16i(val[1]), wrap16i(val[2]), wrap16i(val[3]));
+		return;
+	}
+	int16_t *o = comp + (size_t) blockIdx.x * W + x0;
+	if((W & 3) == 0)
+	{
+		int2 pk;
+		pk.x = (val[0] & 0xFFFF) | (val[1] << 16);
+		pk.y = (val[2] & 0xFFFF) | (val[3] << 16);
+		*reinterpret_cast<int2 *>(o) = pk;
+	}
+	else
+	{
+		#pragma unroll
+		for(int k = 0; k < SPT; k++) if(x0 + k < W) o[k] = (int16_t) val[k];
+	}
+}
+
 // ---------------------------------------------------------------------------
 // Raster kernel: one CTA per scan line, 4 samples per thread -> int16 composite stream
 // (ref video.c:2864-3066 _vid_next_line_raster, vbidata.c:186-239). Low register count
@@ -1178,13 +1244,20 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 				int cu[SPT] = { 0, 0, 0, 0 }, cv[SPT] = { 0, 0, 0, 0 };
 				if(near_pic)
 				{
+					// every tap count a raster up to the kernels' 1536-sample width has (7 at 9 MHz, 17 at 24 MHz); the
+					// lower ones only the --pixelrate raster and the split path run
 					switch(dp.chroma_ntaps)
 					{
+					case 1: chroma_fir4<1>(dp, su, sv, x0, cu, cv); break;
+					case 3: chroma_fir4<3>(dp, su, sv, x0, cu, cv); break;
+					case 5: chroma_fir4<5>(dp, su, sv, x0, cu, cv); break;
+					case 7: chroma_fir4<7>(dp, su, sv, x0, cu, cv); break;
+					case 9: chroma_fir4<9>(dp, su, sv, x0, cu, cv); break;
 					case 11: chroma_fir4<11>(dp, su, sv, x0, cu, cv); break;
 					case 13: chroma_fir4<13>(dp, su, sv, x0, cu, cv); break;
 					case 15: chroma_fir4<15>(dp, su, sv, x0, cu, cv); break;
 					case 17: chroma_fir4<17>(dp, su, sv, x0, cu, cv); break;
-					default:
+					default:                                        // no chroma low-pass (chroma_ntaps = 0)
 						for(int k = 0; k < SPT; k++) { cu[k] = su[x0 + k + UOFF]; cv[k] = sv[x0 + k + UOFF]; }
 					}
 				}
@@ -1217,64 +1290,7 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 			if(li.ov_add >= 0 && x < W) val[k] = wrap16i(val[k]) + dt.ov_add[(size_t) li.ov_add * W + x];
 		}
 	}
-	if(planes && plane_pitch)
-	{
-		// pitched byte planes (htv_mma_fir.h): one self-contained row per line, the first / last
-		// MF_LEAD samples repeated in the halo of the previous / next row of this launch
-		uint8_t *rowp = planes + (size_t) blockIdx.x * plane_pitch;
-		if(x0 + SPT <= W)
-		{
-			*reinterpret_cast<unsigned *>(rowp + MF_LEAD + x0) = ((val[0] >> 8) & 0xFF) | (((val[1] >> 8) & 0xFF) << 8) |
-				(((val[2] >> 8) & 0xFF) << 16) | ((unsigned) (val[3] >> 8) << 24);
-			*reinterpret_cast<unsigned *>(rowp + plane_stride + MF_LEAD + x0) = (val[0] & 0xFF) | ((val[1] & 0xFF) << 8) |
-				((val[2] & 0xFF) << 16) | ((unsigned) val[3] << 24);
-		}
-		const bool head = x0 < MF_LEAD && blockIdx.x > 0, tail = x0 + SPT > W - MF_LEAD && blockIdx.x + 1 < gridDim.x;
-		if(head || tail || x0 + SPT > W)
-		{
-			#pragma unroll
-			for(int k = 0; k < SPT; k++)
-			{
-				const int x = x0 + k;
-				if(x >= W) break;
-				const uint8_t hi = (uint8_t) ((val[k] >> 8) & 0xFF), lo = (uint8_t) (val[k] & 0xFF);
-				if(x0 + SPT > W) { rowp[MF_LEAD + x] = hi; rowp[plane_stride + MF_LEAD + x] = lo; }
-				if(head && x < MF_LEAD) { uint8_t *q = rowp - plane_pitch + MF_LEAD + W + x; q[0] = hi; q[plane_stride] = lo; }
-				if(tail && x >= W - MF_LEAD) { uint8_t *q = rowp + plane_pitch + (x - (W - MF_LEAD)); q[0] = hi; q[plane_stride] = lo; }
-			}
-		}
-		return;
-	}
-	if(planes)
-	{
-		// high / low byte planes for the tensor-core video filter (k_mod_mma): v = 256 hi + lo
-		uint8_t *p = planes + (size_t) blockIdx.x * W + x0;
-		*reinterpret_cast<unsigned *>(p) = ((val[0] >> 8) & 0xFF) | (((val[1] >> 8) & 0xFF) << 8) |
-			(((val[2] >> 8) & 0xFF) << 16) | ((unsigned) (val[3] >> 8) << 24);
-		*reinterpret_cast<unsigned *>(p + plane_stride) = (val[0] & 0xFF) | ((val[1] & 0xFF) << 8) |
-			((val[2] & 0xFF) << 16) | ((unsigned) val[3] << 24);
-		return;
-	}
-	if(comp32)
-	{
-		// int32 stream for the TMA-fed modulator (values are int16-wrapped as the reference's buffer is)
-		*reinterpret_cast<int4 *>(comp32 + (size_t) blockIdx.x * W + x0) =
-			make_int4(wrap16i(val[0]), wrap16i(val[1]), wrap16i(val[2]), wrap16i(val[3]));
-		return;
-	}
-	int16_t *o = comp + (size_t) blockIdx.x * W + x0;
-	if((W & 3) == 0)
-	{
-		int2 pk;
-		pk.x = (val[0] & 0xFFFF) | (val[1] << 16);
-		pk.y = (val[2] & 0xFFFF) | (val[3] << 16);
-		*reinterpret_cast<int2 *>(o) = pk;
-	}
-	else
-	{
-		#pragma unroll
-		for(int k = 0; k < SPT; k++) if(x0 + k < W) o[k] = (int16_t) val[k];
-	}
+	store_line4(val, x0, W, comp, comp32, planes, plane_stride, plane_pitch);
 }
 
 // ---------------------------------------------------------------------------
@@ -3086,12 +3102,13 @@ static int sec_chain(htv_dev_t *d, const LineS2 *ls, int n, cudaStream_t st)
 // R * Wp + floor(k D / I) with the taps of phase (k D) mod I (a whole line is a whole number of
 // periods because Ws D = Wp I). Row b of `comp` is raster line first - 1 + b of the launch; row b
 // of the output is resampled line first + b, which reaches back into comp rows b and b + 1.
-// Output goes wherever the modulator of this context reads: byte planes, int32 or int16 stream.
+// Output goes wherever the modulator of this context reads, in k_raster's store (store_line4): byte planes, pitched
+// or contiguous, int32 or int16 stream.
 // Parity: tests/test_gpu_zz_pixelrate.py against the oracle (itself pinned to the reference's --pixelrate).
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(384)
 k_resample(const int16_t *comp, int Wp, int Ws, int I, int D, int A, const int16_t *taps,
-	uint8_t *planes, size_t plane_stride, int *comp32, int16_t *comp16)
+	uint8_t *planes, size_t plane_stride, int plane_pitch, int *comp32, int16_t *comp16)
 {
 	const int b = blockIdx.x;
 	const int x0 = threadIdx.x * SPT;
@@ -3099,21 +3116,8 @@ k_resample(const int16_t *comp, int Wp, int Ws, int I, int D, int A, const int16
 	const int16_t *in = comp + (size_t) (b + 1) * Wp;                   // input 0 of resampled line first + b
 	int v[SPT];
 	#pragma unroll
-	for(int k = 0; k < SPT; k++) v[k] = rs_output(in, x0 + k, I, D, A, taps);
-	const size_t o = (size_t) b * Ws + x0;
-	if(planes)
-	{
-		*reinterpret_cast<unsigned *>(planes + o) = ((v[0] >> 8) & 0xFF) | (((v[1] >> 8) & 0xFF) << 8) |
-			(((v[2] >> 8) & 0xFF) << 16) | ((unsigned) (v[3] >> 8) << 24);
-		*reinterpret_cast<unsigned *>(planes + plane_stride + o) = (v[0] & 0xFF) | ((v[1] & 0xFF) << 8) |
-			((v[2] & 0xFF) << 16) | ((unsigned) v[3] << 24);
-	}
-	else if(comp32) *reinterpret_cast<int4 *>(comp32 + o) = make_int4(v[0], v[1], v[2], v[3]);
-	else
-	{
-		#pragma unroll
-		for(int k = 0; k < SPT; k++) if(x0 + k < Ws) comp16[o + k] = (int16_t) v[k];
-	}
+	for(int k = 0; k < SPT; k++) v[k] = x0 + k < Ws ? rs_output(in, x0 + k, I, D, A, taps) : 0;
+	store_line4(v, x0, Ws, comp16, comp32, planes, plane_stride, plane_pitch);
 }
 
 // Lines line0 .. line0 + nlines - 1 into d_out. d is the encoder; r is NULL, or with --pixelrate the raster context built
@@ -3129,7 +3133,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, i
 	const DevPlan &p = d->plan;
 	const htv_dparams_t &dp = d->dp;
 	if(nlines <= 0) return(HTV_OK);
-	if((p.path == PATH_RS) != (r != NULL) || (r && (r->plan.path != PATH_RASTER || p.plane_pitch || (dp.W & 3)))) return(HTV_ERROR);
+	if((p.path == PATH_RS) != (r != NULL) || (r && r->plan.path != PATH_RASTER)) return(HTV_ERROR);
 	const bool secam = dp.colour_mode == HTV_SECAM;
 	// FM video with a pre-emphasis filter: the modulator also integrates the pipeline's fill line
 	const int fm_skip = dp.have_fmv && dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
@@ -3158,7 +3162,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, i
 			k_raster<<<n + r->plan.before + r->plan.after, r->plan.line_threads, r->plan.raster_smem, st>>>(r->dp, r->dt,
 				(const LineR2 *) desc_r + done, r->d_comp, NULL, NULL, 0, 0);
 			k_resample<<<rows, p.line_threads, 0, st>>>(r->d_comp, r->dp.W, dp.W, d->rs_I, d->rs_D, d->rs_ataps, d->d_rs_taps,
-				d->d_planes, d->plane_stride, d->d_comp32, d->d_comp);
+				d->d_planes, d->plane_stride, p.plane_pitch, d->d_comp32, d->d_comp);
 			d->launches += 2;
 		}
 		else if(secam)

@@ -51,6 +51,7 @@ def _run(binary, args, nbytes, env=""):
     # --pixelrate: raster at 13.5 MHz, the reference's polyphase resampler on the device, then the usual path
     ("-m i -s 16000000 --pixelrate 13500000 --filter --noaudio", 4, 0),
     ("-m i -s 16000000 --pixelrate 13500000 --filter", 4, 1),
+    ("-m m -s 13500000 --pixelrate 9000000 --filter", 4, 1),          # W = 858 <- 572: pitched byte planes
     # HACKTV_B200_PREFETCH=1: the adapter's vid_next_line runs one frame ahead of the consumer
     ("PREFETCH -m i -s 16000000 --filter", 4, 1),
 ])

@@ -40,6 +40,7 @@ CASES = {
     "secam-W967-real": ("secam", 15109375, 0, {}, {}, False, "k_sec_raster<FULL=0,MAXT=256> + " + KL.format(0, 0, 0, 0, 256, 1)),
     "pal-fm-20M-filter": ("pal-fm", 20000000, 0, F, {}, False, "k_fmv_base<"),
     "i-16M-pixelrate-13M5": ("i", 16000000, 13500000, F, {}, False, "k_raster + k_resample + "),
+    "i-13M5-pixelrate-16M-W864": ("i", 13500000, 16000000, F, {}, False, "k_raster + k_resample + k_mod_mma"),   # pitched
     "i-16M-filter-split": ("i", 16000000, 0, F, {"HTV_PATH": "split"}, False, "k_raster + k_mod"),
     "ntsc-13M5-real-split-W858": ("ntsc", 13500000, 0, {}, {"HTV_PATH": "split"}, False, "k_raster + k_mod"),
     "i-16M-filter-offset-swap": ("i", 16000000, 0, dict(vfilter=True, offset=1250000, swap_iq=True), {}, False, KL.format(1, 1, 1, 0, 256, 0)),

@@ -203,7 +203,7 @@ def test_unpatched_heap_differs_only_near_line_ends(built):
 
 # --pixelrate (SURVEY.md section 8f rank 4): raster at the pixel rate, the reference's polyphase resampler
 # (video.c:3627-3651, fir.c:393-428) to the sample rate in front of the video filter. The oracle restates the
-# rate pairs that keep the line width constant; the CUDA path does not take them yet (htv_init refuses).
+# rate pairs that keep the line width constant; the CUDA path takes them all except SECAM's and FM video's.
 PIXELRATE_CASES = [
     ("pal", 16000000, 13500000, 700, False, ()),                 # 864 -> 1024 samples per line, I/D = 32/27
     ("i", 16000000, 13500000, 700, True, ()),                    # + VSB filter, FM + NICAM two lines ahead
@@ -218,6 +218,22 @@ PIXELRATE_CASES = [
     ("secam", 16000000, 13500000, 400, False, ()),
     ("d", 20000000, 13500000, 300, True, ()),
 ]
+
+
+def _pixelrate_matrix_cases():
+    """Every mode, rate pair and option set the device's --pixelrate path is held at by test_gpu_zz_pixelrate.py, with the
+    mode's sound and the lines it renders: the oracle those tests compare with is the reference there too."""
+    from test_gpu_zz_pixelrate import MATRIX
+    out = []
+    for mode, rate, prate, kw, _, _, _ in MATRIX:
+        extra = tuple(f"--{k}" for k in ("nocolour",) if kw.get(k))
+        case = (mode, rate, prate, 290 if mode in ("m", "ntsc", "pal-m") else 340, bool(kw.get("vfilter")), extra)
+        if case not in PIXELRATE_CASES and case not in out:
+            out.append(case)
+    return out
+
+
+PIXELRATE_CASES += _pixelrate_matrix_cases()
 
 
 @pytest.mark.parametrize("mode,rate,prate,nlines,filt,extra", PIXELRATE_CASES)

@@ -16,7 +16,8 @@ def emu(tmp_path_factory):
     return exe
 
 
-@pytest.mark.parametrize("Wp,I,D", [(864, 32, 27), (864, 40, 27), (1024, 27, 32), (572, 3, 2), (896, 8, 7), (832, 16, 13)])
+@pytest.mark.parametrize("Wp,I,D", [(864, 32, 27), (864, 40, 27), (1024, 27, 32), (572, 3, 2), (896, 8, 7), (832, 16, 13),
+                                    (864, 20, 27), (1280, 4, 5), (865, 1024, 865), (864, 3, 2)])
 def test_closed_form_equals_the_streaming_resampler(emu, Wp, I, D):
     for seed in (1, 2):
         out = subprocess.run([emu, str(Wp), str(I), str(D), str(seed)], capture_output=True, text=True)

@@ -254,6 +254,22 @@ def test_c_selection_runs_what_the_line_width_matrix_asserts(built):
         assert _plan_name(built, mode, 16000000, dict(vfilter=True), HTV_KL="general") == GENERAL
 
 
+def test_c_selection_runs_what_the_pixelrate_matrix_asserts(built):
+    """The GPU pixel-rate matrix (test_gpu_zz_pixelrate.py) without a GPU: every row's W <- Wp is what the tables give,
+    the C selection names the kernels the row asserts, and together the rows reach every split modulator (k_mod_mma,
+    k_mod_tma, k_mod) at both CTA sizes --pixelrate can select."""
+    from test_gpu_zz_pixelrate import MATRIX
+    ran = set()
+    for mode, rate, prate, kw, W, Wp, kernel in MATRIX:
+        t = built.Tables(built.mode_config(mode, **kw), rate, prate)
+        assert (int(t.get("geometry")[0]), int(t.get("rs_geometry")[3])) == (W, Wp), (mode, rate, prate, kw)
+        t.close()
+        assert _plan_name(built, mode, rate, kw, prate) == kernel, (mode, rate, prate, kw)
+        ran.add(kernel)
+    want = {f"k_raster + k_resample + {m}<{t},{b}>" for m in ("k_mod_mma", "k_mod_tma", "k_mod") for t, b in ((256, 4), (384, 2))}
+    assert ran == want, sorted(want ^ ran)
+
+
 def test_c_selection_runs_what_the_sample_type_cases_assert(built):
     """Every case of the GPU sample-type test, for each type: the names it asserts (the split modulators, FM video and
     --pixelrate among them), and the int8 form with PAL's sound stages compiled in, or the general one under HTV_KL=general."""
