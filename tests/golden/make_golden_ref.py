@@ -30,7 +30,8 @@ def main():
         index[key] = {"size": int(a.size), "sha256": hashlib.sha256(a.tobytes()).hexdigest(), **more}
         print(index[key]["sha256"][:16], key)
 
-    def run(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", frames=None, audio=None, ext=None):
+    def run(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", frames=None, audio=None, ext=None,
+            audio_block=4000):
         with tempfile.TemporaryDirectory() as td:
             run_extra = tuple(extra)
             if ext is not None:
@@ -38,7 +39,7 @@ def main():
                 ext.tofile(fn)
                 run_extra += (fn,)                       # the value of the trailing --passthru
             a = orc.run_ref(mode, rate, lines, skip=skip, vfilter=vfilter, extra=run_extra, frames=frames, audio=audio,
-                            audio_block=4000 if audio is not None else 0)
+                            audio_block=audio_block if audio is not None else 0)
         put(T.ref_key(mode, rate, lines, skip=skip, vfilter=vfilter, extra=extra, source=source), a)
         return a
 
@@ -65,6 +66,12 @@ def main():
     o = orc.Oracle(H.mode_config("i", vfilter=True), 16000000)
     frames, audio = T.random_source(7, o.active_lines, o.active_width)
     run("i", 16000000, 1400, vfilter=True, source="random7", frames=frames, audio=audio)
+
+    for mode, rate, filt, extra, nlines, block, seed in T.programme_cases():
+        o = orc.Oracle(T._conf(H, mode, filt, extra), rate)
+        frames, audio = T.programme_source(seed, o.active_lines, o.active_width)
+        run(mode, rate, nlines, vfilter=filt, extra=extra, source=f"programme{seed}", frames=frames, audio=audio,
+            audio_block=block)
 
     raw = orc.run_ref("i", 16000000, 700, vfilter=True, rawheap=True)
     put(T.ref_key("i", 16000000, 700, vfilter=True, rawheap=True), raw,

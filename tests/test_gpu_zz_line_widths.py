@@ -113,14 +113,14 @@ def _env(**env):
                 os.environ[k] = v
 
 
-def _render(H, conf, rate, pieces, frames=None, audio=None, **env):
+def _render(H, conf, rate, pieces, frames=None, audio=None, audio_block=0, **env):
     """The CUDA path's stream over calls of `pieces` lines, and the line kernel it ran."""
     with _env(**env):
         enc = H.Encoder(conf, rate)
     if frames is None:
         enc.open_test_source()
     else:
-        enc.set_source(frames, audio)
+        enc.set_source(frames, audio, audio_block=audio_block)
     got = np.concatenate([enc.render_host(n) for n in pieces])
     name = enc.line_kernel
     enc.close()
@@ -227,7 +227,7 @@ def test_wide_lines_random_pictures_loud_audio_and_uneven_calls(built, mode, rat
     assert np.array_equal(whole, parts)
 
 
-@pytest.mark.parametrize("mode", ["i", "b"])
+@pytest.mark.parametrize("mode", ["i", "b", "pal-d"])
 def test_compiled_in_sound_form_equals_the_general_form(built, mode):
     """The instantiation with PAL's VSB + FM + NICAM stages and W = 1024 compiled in (16 Msps) against the general one
     (HTV_KL=general): bit-identical on the test card, on random pictures with full-scale noise audio, and over calls of

@@ -70,7 +70,19 @@ def _line_width_cases():
     return out
 
 
+def _mode_matrix_cases():
+    """Every row of the device's mode matrix (test_gpu_zz_modes.py), with the mode's sound and the lines it renders."""
+    from test_gpu_zz_modes import MATRIX
+    out = []
+    for mode, rate, kw, _, _ in MATRIX:
+        case = (mode, rate, 1100 if mode in ("ntsc-i", "pal60-i", "pal60", "525pal") else 1300, bool(kw.get("vfilter")), ())
+        if case not in CASES and case not in out:
+            out.append(case)
+    return out
+
+
 CASES += _line_width_cases()
+CASES += _mode_matrix_cases()
 
 
 def ref_key(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", rawheap=False):
@@ -104,6 +116,30 @@ def random_source(seed, active_lines, active_width):
     return frames, audio
 
 
+def programme_source(seed, active_lines, active_width):
+    """Three random pictures and 2 711 stereo sound samples (an odd number, so that the loop's wrap falls inside an
+    audio block) that reach the edges of the input range within the first 2 220, about 1 090 lines:
+       0 ..  200  silence
+     200 ..  900  uniform noise over the whole range, +32767 and -32768 included
+     900 .. 1320  a full-scale square wave of period 4 .. 8 on both channels: through pre-emphasis it drives the FM
+                  limiter hard
+    1320 .. 1720  L = 2k + 1, R = -(2k + 2): L + R = -1, where the mono mix truncates toward zero
+    1720 .. 1970  DC at -32768, then to 2 220 at +32767; after that noise again up to the wrap."""
+    rng = np.random.default_rng(seed)
+    frames = rng.integers(0, 1 << 24, size=(3, active_lines, active_width), dtype=np.uint32)
+    audio = np.zeros((2711, 2), dtype=np.int16)
+    audio[200:900] = rng.integers(-32768, 32767, size=(700, 2), endpoint=True)
+    audio[200], audio[201] = (32767, -32768), (-32768, 32767)
+    square = np.concatenate([np.where(np.arange(p) < p // 2, 32767, -32768) for p in np.tile(np.arange(4, 9), 14)])
+    audio[900:1320] = square[:, None]
+    k = rng.integers(-16384, 16383, size=400, endpoint=True)
+    audio[1320:1720, 0], audio[1320:1720, 1] = 2 * k + 1, -(2 * k + 2)
+    audio[1720:1970] = -32768
+    audio[1970:2220] = 32767
+    audio[2220:] = rng.integers(-32768, 32767, size=(491, 2), endpoint=True)
+    return frames, audio
+
+
 def _conf(H, mode, filt, extra):
     kw = dict(vfilter=filt)
     it = iter(extra)
@@ -113,6 +149,7 @@ def _conf(H, mode, filt, extra):
         elif e == "--nocolour": kw["nocolour"] = True
         elif e == "--swap-iq": kw["swap_iq"] = True
         elif e == "--offset": kw["offset"] = int(next(it))
+        elif e == "--volume": kw["volume"] = float(next(it))
     return H.mode_config(mode, **kw)
 
 
@@ -188,6 +225,27 @@ def test_oracle_equals_reference_on_random_input(built):
     got = o.render(1400)
     o.close()
     assert_reference(got, ref_key("i", 16000000, 1400, vfilter=True, source="random7"))
+
+
+def programme_cases():
+    """The programme-audio runs of the device (test_gpu_zz_modes.py): (mode, rate, vfilter, extra options, lines,
+    audio block, seed)."""
+    from test_gpu_zz_modes import PROGRAMME, PROGRAMME_BLOCK, PROGRAMME_LINES, PROGRAMME_SEED
+    out = []
+    for mode, rate, kw in PROGRAMME:
+        extra = ("--volume", f"{kw['volume']:g}") if "volume" in kw else ()
+        out.append((mode, rate, bool(kw.get("vfilter")), extra, PROGRAMME_LINES, PROGRAMME_BLOCK, PROGRAMME_SEED))
+    return out
+
+
+@pytest.mark.parametrize("mode,rate,filt,extra,nlines,block,seed", programme_cases())
+def test_oracle_equals_reference_on_programme_audio(built, mode, rate, filt, extra, nlines, block, seed):
+    """programme_source read in blocks of `block` pairs by the reference; the oracle takes it whole."""
+    o = orc.Oracle(_conf(built, mode, filt, extra), rate)
+    o.set_source(*programme_source(seed, o.active_lines, o.active_width))
+    got = o.render(nlines)
+    o.close()
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=filt, extra=extra, source=f"programme{seed}"))
 
 
 def test_unpatched_heap_differs_only_near_line_ends(built):

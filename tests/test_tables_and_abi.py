@@ -249,9 +249,51 @@ def test_c_selection_runs_what_the_line_width_matrix_asserts(built):
     from test_gpu_zz_line_widths import FIXED, GENERAL, MATRIX
     for mode, rate, kw, _, kernel in MATRIX:
         assert _plan_name(built, mode, rate, kw) == kernel, (mode, rate, kw)
-    for mode in ("i", "b"):
+    for mode in ("i", "b", "pal-d"):
         assert _plan_name(built, mode, 16000000, dict(vfilter=True)) == FIXED
         assert _plan_name(built, mode, 16000000, dict(vfilter=True), HTV_KL="general") == GENERAL
+
+
+def test_c_selection_runs_what_the_mode_matrix_asserts(built):
+    """The GPU mode matrix (test_gpu_zz_modes.py) without a GPU: every row's W is what the tables give, and the C
+    selection names the kernels the row asserts - the tables' own choice, or the form with PAL's sound stages compiled in
+    where the tables' choice is its general form."""
+    from test_gpu_zz_line_widths import FIXED, GENERAL
+    from test_gpu_zz_modes import MATRIX
+    for mode, rate, kw, W, kernel in MATRIX:
+        w, _, _, _, sel = _line_kernel_from_tables(built, mode, rate, kw)
+        what = f"{mode} {rate} {kw}"
+        assert w == W, (what, w)
+        assert sel == (GENERAL if kernel == FIXED else kernel), (what, sel)
+        assert _plan_name(built, mode, rate, kw) == kernel, what
+
+
+def test_aliases_are_their_base_modes(built):
+    """g, k, pal-k and secam-g are other names of b, d, pal-d and secam-b: byte-identical configurations. No two other
+    ids share one, so the list of aliases is complete."""
+    from test_gpu_zz_modes import ALIASES
+    m = built.modes()
+    raw = {k: bytes(c) for k, (c, _) in m.items()}
+    for alias, base in ALIASES.items():
+        assert raw[alias] == raw[base], (alias, base)
+        assert m[alias][1] == m[base][1], (alias, base)
+    same = {(a, b) for a in raw for b in raw if a < b and raw[a] == raw[b]}
+    assert same == {tuple(sorted(p)) for p in ALIASES.items()}, sorted(same)
+
+
+def test_every_mode_is_rendered_on_the_device(built):
+    """Every id the encoder accepts is rendered against the oracle by a GPU matrix - the mode matrix, the line-width or
+    pixel-rate matrix, or the parity cases - or is an alias of one that is. A mode added without a device test fails here."""
+    from test_gpu_parity import CASES as PARITY
+    from test_gpu_zz_line_widths import MATRIX as WIDTHS
+    from test_gpu_zz_modes import ALIASES, MATRIX as MODES
+    from test_gpu_zz_pixelrate import MATRIX as PIXELRATE
+    rendered = {c[0] for c in MODES + WIDTHS + PIXELRATE + PARITY}
+    ids = set(built.modes())
+    assert not rendered - ids, sorted(rendered - ids)
+    missing = {i for i in ids if i not in rendered and ALIASES.get(i) not in rendered}
+    assert not missing, sorted(missing)
+    assert set(ALIASES) <= ids and not set(ALIASES) & {c[0] for c in MODES}
 
 
 def test_c_selection_runs_what_the_pixelrate_matrix_asserts(built):
