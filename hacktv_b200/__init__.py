@@ -63,7 +63,7 @@ class Config(C.Structure):
         ("burst_level", C.c_double), ("burst_rise", C.c_double),
         ("ev_co", C.c_double), ("eu_co", C.c_double),
         ("fm_mono_carrier", C.c_double), ("fm_mono_deviation", C.c_double),
-        ("fm_mono_preemph", C.c_int32), ("reserved0", C.c_int32),
+        ("fm_mono_preemph", C.c_int32), ("s_video", C.c_int32),
         ("nicam_carrier", C.c_double), ("nicam_beta", C.c_double), ("am_mono_carrier", C.c_double),
         ("fm_level", C.c_double), ("fm_deviation", C.c_double), ("fm_energy_dispersal", C.c_double),
     ]
@@ -198,8 +198,10 @@ def modes() -> dict:
 
 
 def mode_config(mode: str, *, vfilter=False, nocolour=False, noaudio=False, nonicam=False,
-                offset=0, swap_iq=False, level=1.0, volume=1.0, invert_video=False, deviation=0.0) -> Config:
-    """Mode lookup + the command-line overrides of reference hacktv.c:1107-1437 (in-scope options)."""
+                offset=0, swap_iq=False, level=1.0, volume=1.0, invert_video=False, deviation=0.0,
+                s_video=False) -> Config:
+    """Mode lookup + the command-line overrides of reference hacktv.c:1107-1437 (in-scope options). s_video sets the
+    field as --s-video does; whether the mode allows it is htv_init's check (hacktv.c:1136-1148)."""
     p = lib().htv_find_mode(mode.encode())
     if not p:
         raise ValueError(f"Unrecognised TV mode {mode!r}")
@@ -221,6 +223,7 @@ def mode_config(mode: str, *, vfilter=False, nocolour=False, noaudio=False, noni
     c.invert_video = int(bool(invert_video))
     if deviation > 0:
         c.fm_deviation = float(deviation)            # -D / --deviation, hacktv.c:1109-1113
+    c.s_video = int(bool(s_video))
     return c
 
 

@@ -30,6 +30,7 @@ static void usage(void)
 		"  -t, --type <type>      Sample type: uint8, int8, uint16, int16 (default), int32, float\n"
 		"      --filter           Enable the VSB / low-pass video filter\n"
 		"      --nocolour --noaudio --nonicam --swap-iq\n"
+		"      --s-video          Chroma on Q, luma on I (PAL, SECAM or NTSC baseband modes; the file is I,Q)\n"
 		"      --offset <hz>  --level <f>  --volume <f>\n"
 		"      --lines <n>        Stop after n scan lines (default: run until interrupted)\n");
 }
@@ -38,7 +39,7 @@ int main(int argc, char **argv)
 {
 	const char *mode = "i", *out = NULL, *input = NULL;
 	unsigned int rate = 16000000, pixelrate = 0;   /* --pixelrate: raster at this rate, resampled to -s (not yet run on a GPU) */
-	int filter = 0, nocolour = 0, noaudio = 0, nonicam = 0, swap_iq = 0, type = HTV_TYPE_INT16, i;
+	int filter = 0, nocolour = 0, noaudio = 0, nonicam = 0, swap_iq = 0, s_video = 0, type = HTV_TYPE_INT16, i;
 	long long offset = 0, lines = -1, n = 0;
 	double level = 1.0, volume = 1.0;
 	const htv_config_t *mc;
@@ -64,6 +65,7 @@ int main(int argc, char **argv)
 		else if(!strcmp(a, "--noaudio")) noaudio = 1;
 		else if(!strcmp(a, "--nonicam")) nonicam = 1;
 		else if(!strcmp(a, "--swap-iq")) swap_iq = 1;
+		else if(!strcmp(a, "--s-video")) s_video = 1;
 		else if(!strcmp(a, "--offset") && i + 1 < argc) offset = strtoll(argv[++i], NULL, 10);
 		else if(!strcmp(a, "--level") && i + 1 < argc) level = atof(argv[++i]);
 		else if(!strcmp(a, "--volume") && i + 1 < argc) volume = atof(argv[++i]);
@@ -88,6 +90,17 @@ int main(int argc, char **argv)
 	if(nocolour && (conf.colour_mode == HTV_PAL || conf.colour_mode == HTV_SECAM || conf.colour_mode == HTV_NTSC))
 	{
 		conf.colour_mode = HTV_MONOCHROME;
+	}
+	if(s_video)
+	{
+		/* ref hacktv.c:1136-1148 */
+		if((conf.colour_mode != HTV_PAL && conf.colour_mode != HTV_SECAM && conf.colour_mode != HTV_NTSC) ||
+		   conf.output_type != HTV_INT16_REAL)
+		{
+			fprintf(stderr, "S-Video is only available with PAL, SECAM, or NTSC baseband modes.\n");
+			return(-1);
+		}
+		conf.s_video = 1;
 	}
 	if(noaudio)
 	{

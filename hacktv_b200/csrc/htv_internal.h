@@ -65,7 +65,10 @@ typedef struct {
 	int32_t have_am, am_level;
 	uint64_t am_ang;               /* carrier step, turns * 2^64 */
 	int32_t have_nicam, nicam_ntaps, nicam_F, nicam_D, nicam_cc_len, nicam_tpad_len;
-	int32_t nicam_sps, nicam_minor_short, nicam_lut_ok, nicam_pad2;
+	int32_t nicam_sps, nicam_minor_short, nicam_lut_ok;
+	/* S-Video: the colour subcarrier goes to Q (k_line KL_SV); in what was this block's padding word, so that no field
+	 * moves */
+	int32_t s_video;
 
 	/* SECAM */
 	int32_t secam_level, secam_dmin[2], secam_dmax[2], secam_pad;

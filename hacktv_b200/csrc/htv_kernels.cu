@@ -233,6 +233,7 @@ struct htv_dev_t {
 	int16_t *d_rs_taps;
 	int mod_grid;                     // persistent CTAs of k_mod_tma / k_mod_mma
 	int16_t *d_comp;                  // composite scratch, (sub + 3) lines, reused by every sub-batch (stays in L2)
+	int16_t *d_compq;                 // SECAM with S-Video: the rows' Q (the subcarrier), beside d_comp; NULL otherwise
 	int sub_lines;
 	int last_mod_lines;
 };
@@ -2190,7 +2191,8 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 // resident CTAs per SM of a persistent line kernel of MAXT threads
 #define KL_MINB(T) ((T) <= 256 ? KL_B256 : (T) <= 320 ? KL_B320 : KL_B384)
 
-typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, int, int, int16_t *, const int16_t *, int, const int16_t *);
+typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, int, int, int16_t *, const int16_t *, int, const int16_t *,
+	const int16_t *);
 struct KLine { KLineFn fn; int vf, hq, full, csat, maxt, minb, src, snd, wc, st; };
 #define KL_ENTRY(VF, HQ, FU, CS, T, SRC, SND, WC, ST) \
 	{ k_line<VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST>, VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST }
@@ -2246,13 +2248,15 @@ template<typename E, size_t N, typename F> static const E *kfind(const E (&tab)[
 }
 
 // The name of a k_line instantiation, every template argument spelled out (htv_line_kernel). The int16 forms keep their
-// names; a store that converts appends its sample type: ",ST=int8" compiled in, ",ST=-1:float" converting at run time.
-static void kl_name(char *s, size_t n, const KLine &k, int type)
+// names; a store that converts appends its sample type: ",ST=int8" compiled in, ",ST=-1:float" converting at run time;
+// the S-Video form (KL_SV at run time) appends ",SV".
+static void kl_name(char *s, size_t n, const KLine &k, int type, bool sv)
 {
 	char ts[24] = "";
 	if(k.st < 0) snprintf(ts, sizeof(ts), ",ST=-1:%s", htv_st_name(type));
 	else if(k.st != HTV_TYPE_INT16) snprintf(ts, sizeof(ts), ",ST=%s", htv_st_name(k.st));
-	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d%s>", k.vf, k.hq, k.full, k.csat, k.maxt, k.src, k.snd, k.wc, ts);
+	snprintf(s, n, "k_line<VF=%d,HQ=%d,FULL=%d,CSAT=%d,MAXT=%d,SRC=%d,SND=%d,WC=%d%s%s>", k.vf, k.hq, k.full, k.csat, k.maxt, k.src, k.snd,
+		k.wc, ts, sv ? ",SV" : "");
 }
 
 // ---------------------------------------------------------------------------
@@ -2378,6 +2382,17 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	else if(secam && !sw.split) p->path = PATH_SEC_LINE;
 	else if(!secam && !sw.split && chroma_ok && (!dp.vf_type || mma)) p->path = PATH_LINE;
 	else p->path = PATH_SPLIT;
+	// S-Video has a form in the fused line kernels only (k_line KL_SV, k_sec_raster + k_sec_out's Q plane)
+	if(dp.s_video && ((p->path != PATH_LINE && p->path != PATH_SEC_LINE) || (secam && sw.scalar)))
+	{
+		char why[96];
+		if(sw.split) snprintf(why, sizeof(why), "HTV_PATH=split selects the split modulators");
+		else if(sw.scalar) snprintf(why, sizeof(why), "HTV_FIR=scalar selects the scalar %s", secam ? "SECAM notch" : "video filter");
+		else if(!chroma_ok) snprintf(why, sizeof(why), "a chroma low-pass of %d taps (k_line takes 3 .. 17) runs on the split modulators", dp.chroma_ntaps);
+		else snprintf(why, sizeof(why), "path %d", p->path);
+		snprintf(err, errlen, "S-Video runs on the fused line kernels only: %s", why);
+		return(HTV_ERROR);
+	}
 	// The lines a call rasters around the ones it emits, for the raster descriptors, the raster stage and the row the
 	// modulators read from: one on either side, which the video filter and the line kernels look into. SECAM's rows
 	// reach one line further back. The pixel-rate raster reaches one line further on: emitted line t is resampled line
@@ -2466,8 +2481,10 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	snprintf(tail, sizeof(tail), typed ? " ST=-1:%s" : "", htv_st_name(type));
 	if(p->kl)
 	{
-		kl_name(kl, sizeof(kl), *p->kl, type);
+		kl_name(kl, sizeof(kl), *p->kl, type, dp.s_video);
 		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 + ntp + 128;
+		// S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
+		if(dp.s_video && p->path == PATH_LINE) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
 	}
 	if(p->path == PATH_LINE) snprintf(p->kname, sizeof(p->kname), "%s", kl);
 	else if(p->ks) snprintf(p->kname, sizeof(p->kname), "%s<FULL=%d,MAXT=%d> + %s", rname, p->ks->full, p->ks->maxt, kl);
@@ -2477,7 +2494,9 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	return(HTV_OK);
 }
 
-// Gives each kernel of the plan the dynamic shared memory it launches with
+// Gives each kernel of the plan the dynamic shared memory it launches with. The limit belongs to the function, which every
+// encoder in the process shares, and encoders of one instantiation ask for different amounts (the NICAM pulse table,
+// S-Video's chroma rows): it is only ever raised, so that an encoder created later cannot lower it under an earlier one.
 static bool plan_attributes(const DevPlan &p, char *err, size_t errlen)
 {
 	const KMod *m = p.mod;
@@ -2490,7 +2509,11 @@ static bool plan_attributes(const DevPlan &p, char *err, size_t errlen)
 	};
 	for(const auto &e : k)
 	{
-		const cudaError_t r = e.fn ? cudaFuncSetAttribute(e.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) e.smem) : cudaSuccess;
+		if(!e.fn) continue;
+		cudaFuncAttributes fa;
+		cudaError_t r = cudaFuncGetAttributes(&fa, e.fn);
+		if(r == cudaSuccess && (size_t) fa.maxDynamicSharedSizeBytes < e.smem)
+			r = cudaFuncSetAttribute(e.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) e.smem);
 		if(r != cudaSuccess) { snprintf(err, errlen, "%s: %zu bytes of shared memory refused (%s)", p.kname, e.smem, cudaGetErrorString(r)); return(false); }
 	}
 	return(true);
@@ -2632,6 +2655,8 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	const size_t rows = (size_t) d->sub_lines + 3;       // every path's before + after is at most 3 (plan_kernels)
 	if(p.path != PATH_LINE && cudaMalloc((void **) &d->d_comp, sizeof(int16_t) * rows * W + 256) != cudaSuccess)
 		return(create_fail(d, err, errlen, "device allocation failed"));
+	if(secam && dp.s_video && cudaMalloc((void **) &d->d_compq, sizeof(int16_t) * rows * W + 256) != cudaSuccess)
+		return(create_fail(d, err, errlen, "device allocation failed"));
 	if(p.path == PATH_FMV)
 	{
 		dt.fmv_base = (int16_t *) dev_zero(d, sizeof(int16_t) * (rows + 1) * W + 256);
@@ -2733,7 +2758,7 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	// the side streams may still be ahead of the caller's; nothing of this encoder is freed under running work
 	cudaDeviceSynchronize();
 	for(int i = 0; i < d->nalloc; i++) cudaFree(d->alloc[i]);
-	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_comp); cudaFree(d->d_comp32); cudaFree(d->d_planes);
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_comp); cudaFree(d->d_compq); cudaFree(d->d_comp32); cudaFree(d->d_planes);
 	if(d->h_map) cudaFreeHost(d->h_map);
 	if(d->h_ov_line) { cudaFreeHost(d->h_ov_line); cudaFreeHost(d->h_ov_meta); cudaFreeHost(d->h_ov_add); }
 	cudaFree(d->d_ov_line); cudaFree(d->d_ov_meta); cudaFree(d->d_ov_add);
@@ -3088,7 +3113,7 @@ static int sec_chain(htv_dev_t *d, const LineS2 *ls, int n, cudaStream_t st)
 	}
 	if((pass - 1) & 1) cs.final_odd++; else cs.final_even++;
 	k_sec_carry<<<1, 32, 0, st>>>(ls, d->sec, n - 1, pass - 1);
-	k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, ls, d->sec, d->d_comp, nch);
+	k_sec_out<<<dim3((d->dp.W + 63) / 64, (nch + 31) / 32), 256, 0, st>>>(d->dp, d->dt, ls, d->sec, d->d_comp, nch, d->d_compq);
 	d->launches += 2;
 	return(HTV_OK);
 }
@@ -3203,7 +3228,7 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, i
 			const int grid = persistent_grid(n, d->kl_ctas, &run);
 			const bool line = p.path == PATH_LINE;
 			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, line ? (const LineR2 *) desc_r : NULL, la2 + done, n, run,
-				o, acc, acc_rows, line ? NULL : d->d_comp);
+				o, acc, acc_rows, line ? NULL : d->d_comp, line ? NULL : d->d_compq);
 			if(line)
 			{
 				// this call's descriptor buffers are free again once ev_kl has passed; the next call takes the other two

@@ -112,15 +112,21 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 // chrominance chain (htv_secam.cuh) runs between the raster and the modulator. R1b / R2 fold away, the rest is the same.
 // WC: the line width compiled in (0: dp.W), so that the shared-memory row and plane offsets become immediates
 // ST: the output sample type compiled into the store (HTV_TYPE_INT16: the int16 store), -1: dp.sample_type at run time
+//
+// S-Video (KL_SV, dp.s_video; ref video.c:3031-3040, 3206-3228): the subcarrier term of R2 goes to Q instead of I, and the
+// video filter runs on I only, so Q of the stored line is that line's own chroma. R2 parks it in a two-row ring in shared
+// memory at the lane's own slots (row q & 1), M takes it back for mrow: no other thread touches the slots, so no barrier
+// orders them, and nothing stays live in registers across the loop. SRC: the chain wrote Q into its own plane, `srcq`.
 template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap,
-	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr)
+	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr, const int16_t *srcq = nullptr)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = WC ? WC : dp.W;
 	const int RB = kl_row_bytes(W), UB = kl_uv_bytes(W);
-	// descriptors x2 | [row 0..2][hi, lo] composite planes | [u hi, u lo, v hi, v lo] | FIR taps | chroma taps | NICAM pulse
+	// descriptors x2 | [row 0..2][hi, lo] composite planes | [u hi, u lo, v hi, v lo] | FIR taps | chroma taps | NICAM pulse |
+	// S-Video chroma [row 0..1][j][thread]
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
 	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + 2);
 	unsigned char *rows = reinterpret_cast<unsigned char *>(slr + 2);
@@ -131,6 +137,8 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	const int tid = threadIdx.x, lane = tid & 31, nt = tid >> 5;
 	const int g = lane >> 2, t = lane & 3;
 	const int xb = mf_lane_x(nt, lane, 0);                                  // the lane's samples: xb + 8 j
+	const bool sv = KL_HAS(SND, KL_SV, dp.s_video);
+	short *const svq = ntp + ((dp.nicam_tpad_len + 7) & ~7);
 
 	const int a = blockIdx.x * run, bnd = min(a + run, nlines);
 	if(a >= nlines) return;
@@ -199,6 +207,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		const int li_al = SRC ? 0 : li.al, li_ar = SRC ? 0 : li.ar, li_pal = SRC ? 0 : li.pal;
 		int val[4] = { tm[0], tm[1], tm[2], tm[3] };
 		int uu[4] = { 0, 0, 0, 0 }, vv[4] = { 0, 0, 0, 0 };
+		int cq[4] = { 0, 0, 0, 0 };                                         // S-Video: the chroma of line q
 		if(in_full && li_al < li_ar)
 		{
 			if(xb >= li_al && xb + 24 < li_ar && !li.keep)
@@ -295,8 +304,21 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 					}
 				}
 			}
+			if(sv)
+			{
+				#pragma unroll
+				for(int j = 0; j < 4; j++) cq[j] = ((int) cl[j].x * cv[j] * li_pal + (int) cl[j].y * cu[j]) >> 15;
+			}
+			else
+			{
+				#pragma unroll
+				for(int j = 0; j < 4; j++) val[j] += ((int) cl[j].x * cv[j] * li_pal + (int) cl[j].y * cu[j]) >> 15;
+			}
+		}
+		if(!SRC && sv)
+		{
 			#pragma unroll
-			for(int j = 0; j < 4; j++) val[j] += ((int) cl[j].x * cv[j] * li_pal + (int) cl[j].y * cu[j]) >> 15;
+			for(int j = 0; j < 4; j++) svq[((q & 1) * 4 + j) * blockDim.x + tid] = (short) cq[j];
 		}
 		if(!SRC && li.ov_any)
 		{
@@ -386,6 +408,17 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		// ---- sound carriers, mixers, store ---------------------------------------
 		if(FULL || xb < W)
 		{
+			if(sv)
+			{
+				// Q = the chroma of line mrow (the video filter leaves it alone)
+				const int16_t *qp = srcq + (size_t) (mrow + 2) * W + xb;
+				#pragma unroll
+				for(int j = 0; j < 4; j++)
+				{
+					if(SRC) oq[j] += (FULL || xb + 8 * j < W) ? (int) __ldg(qp + 8 * j) : 0;
+					else oq[j] += svq[((mrow & 1) * 4 + j) * blockDim.x + tid];
+				}
+			}
 			const LineA2 *la = sla + (mrow & 1);
 			kl_sound<SND, 8>(dp, dt, la, ntp, xb, oi, oq);
 			kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);

@@ -565,9 +565,11 @@ __global__ void k_sec_carry(const LineS2 *lr, SecScratch ss, int idx, int pass_f
 
 // After the fixed point: subcarrier samples from (FM input, phasor) - bell gain, level, burst window (ref
 // video.c:3216-3228) - added to the composite rows in place, for 32 lines x 64 samples per CTA: read from the transposed
-// arrays lane = line, exchanged through shared memory, added row-wise.
+// arrays lane = line, exchanged through shared memory, added row-wise. S-Video: `compq` is not NULL, and every row of it
+// is written instead (Q; zero where a line has no subcarrier).
 __global__ void __launch_bounds__(256)
-k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int16_t *comp, int nchain)
+k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineS2 *lr, SecScratch ss, int16_t *comp, int nchain,
+	int16_t *compq)
 {
 	__shared__ __align__(16) short tile[32][64 + 8];
 	__shared__ int any[32];
@@ -617,7 +619,13 @@ k_sec_out(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	__syncthreads();
 	{
 		const int l = threadIdx.x >> 3, q = threadIdx.x & 7, c = r0 + l, x = xt + q * 8;
-		if(c < nchain && x < W && any[l])
+		if(compq && c < nchain && x < W)
+		{
+			int16_t *dst = compq + (size_t) c * W + x;
+			if((W & 7) == 0) *reinterpret_cast<int4 *>(dst) = *reinterpret_cast<const int4 *>(&tile[l][q * 8]);
+			else for(int k = 0; k < 8 && x + k < W; k++) dst[k] = tile[l][q * 8 + k];
+		}
+		else if(c < nchain && x < W && any[l])
 		{
 			int16_t *dst = comp + (size_t) c * W + x;
 			if((W & 7) == 0)

@@ -8,7 +8,7 @@
 // accumulators land on the lane's own four samples, the next line's template and pixels are fetched while this line's
 // filters run, and there is one barrier per line (byte planes double-buffered). Lines do not depend on each other.
 // Outputs as before: composite rows (int16, luma only - k_sec_out adds the subcarrier), the baseband in the chain's
-// transposed layout, the raw sums of the last 7 low-pass outputs.
+// transposed layout, the raw sums of the last 7 low-pass outputs. S-Video (dp.s_video) skips the notch (ref video.c:3206).
 
 template<bool FULL, int MAXT, int MINB>
 __global__ void __launch_bounds__(MAXT, MINB)
@@ -139,7 +139,7 @@ k_sec_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const
 
 		if(proc)
 		{
-			if(notch_tile)
+			if(notch_tile && !dp.s_video)
 			{
 				// ---- luma notch over the picture: 51 taps, three k-steps of 32 ----------
 				const unsigned char *ph = lum + (2 * b) * RB + fo0, *plo = ph + RB;

@@ -21,13 +21,14 @@ __device__ __forceinline__ short2 kl_ldc16(const htv_c16_t *p) { return(__ldg(re
 #define KL_OFF  8
 #define KL_SWAP 16
 #define KL_CPX  32
+#define KL_SV   64      // S-Video: the colour subcarrier goes to Q (k_line only; no compiled-in mask has it)
 #define KL_SND_FM_NICAM (KL_FM | KL_NIC | KL_CPX)
 #define KL_HAS(SND, BIT, RT) ((SND) < 0 ? (RT) != 0 : ((SND) & (BIT)) != 0)
 
 static inline int kl_snd_mask(const htv_dparams_t &dp)
 {
 	return((dp.have_fm ? KL_FM : 0) | (dp.have_am ? KL_AM : 0) | (dp.have_nicam ? KL_NIC : 0) |
-		(dp.have_offset ? KL_OFF : 0) | (dp.swap_iq ? KL_SWAP : 0) | (dp.complex_out ? KL_CPX : 0));
+		(dp.have_offset ? KL_OFF : 0) | (dp.swap_iq ? KL_SWAP : 0) | (dp.complex_out ? KL_CPX : 0) | (dp.s_video ? KL_SV : 0));
 }
 
 // ---- sound carriers for the four samples xb + S j of a thread, added into oi / oq -------------------------------

@@ -352,6 +352,18 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 		fprintf(stderr, "hacktv_b200: FM energy dispersal is not on the accelerated path\n");
 		return(NULL);
 	}
+	if(conf->s_video && ((conf->colour_mode != HTV_PAL && conf->colour_mode != HTV_SECAM && conf->colour_mode != HTV_NTSC) ||
+	   conf->output_type != HTV_INT16_REAL))
+	{
+		/* ref hacktv.c:1136-1148 */
+		fprintf(stderr, "S-Video is only available with PAL, SECAM, or NTSC baseband modes.\n");
+		return(NULL);
+	}
+	if(conf->s_video && conf->modulation != HTV_NONE)
+	{
+		fprintf(stderr, "hacktv_b200: S-Video with a modulated carrier is not on the accelerated path\n");
+		return(NULL);
+	}
 
 	t = calloc(1, sizeof(*t));
 	if(!t) return(NULL);
@@ -380,7 +392,9 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 	dp->active_lines = c->active_lines;
 	dp->raster = c->type;
 	dp->colour_mode = c->colour_mode;
-	dp->complex_out = c->output_type == HTV_INT16_COMPLEX;
+	/* S-Video: luma on I, chroma on Q; the file sink writes both (ref hacktv.c:1493) */
+	dp->s_video = c->s_video != 0;
+	dp->complex_out = c->output_type == HTV_INT16_COMPLEX || dp->s_video;
 	dp->sample_type = HTV_TYPE_INT16;
 	dp->interlaced = c->interlaced;
 	dp->volume = c->volume;
@@ -814,6 +828,12 @@ htv_tables_t *htv_tables_create2(const htv_config_t *conf, unsigned int sample_r
 	if(conf->modulation == HTV_FM)
 	{
 		fprintf(stderr, "hacktv_b200: --pixelrate with FM video is not on the accelerated path\n");
+		return(NULL);
+	}
+	if(conf->s_video)
+	{
+		/* the resampler would run on two channels (ref video.c:4362-4368) */
+		fprintf(stderr, "hacktv_b200: --pixelrate with S-Video is not on the accelerated path\n");
 		return(NULL);
 	}
 	t = htv_tables_create(conf, sample_rate);

@@ -122,7 +122,12 @@ typedef struct {
 	double fm_mono_carrier;
 	double fm_mono_deviation;
 	int32_t fm_mono_preemph;
-	int32_t reserved0;
+	/* S-Video (ref video.h:229, --s-video hacktv.c:1136-1148): luma and sync on I, the colour subcarrier and its burst
+	 * on Q instead of added to I; the stream is then complex (htv_is_complex). PAL, NTSC and SECAM colour with
+	 * output_type HTV_INT16_REAL and no modulation only; not with a pixel rate other than the sample rate. It takes
+	 * what was this struct's padding word, so that the layout (and orc_params_t's, which keeps the word as padding)
+	 * does not change */
+	int32_t s_video;
 	double nicam_carrier;
 	double nicam_beta;
 	double am_mono_carrier;

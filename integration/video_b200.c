@@ -58,7 +58,7 @@ static int _accelerated(const vid_config_t *c, unsigned int sample_rate, unsigne
 	if(c->type != VID_RASTER_625 && c->type != VID_RASTER_525) return(0);
 	if(c->modulation == VID_FM && c->fm_energy_dispersal != 0) return(0);
 	if(c->colour_mode != VID_NONE && c->colour_mode != VID_PAL && c->colour_mode != VID_NTSC && c->colour_mode != VID_SECAM) return(0);
-	/* --pixelrate: PAL / NTSC / mono through the device resampler; SECAM and FM video with a resampler,
+	/* --pixelrate: PAL / NTSC / mono through the device resampler; SECAM, FM video and S-Video with a resampler,
 	 * and rate pairs whose line width would vary, stay on the stock encoder (DESIGN.md section 8) */
 	if(pixel_rate && pixel_rate != sample_rate)
 	{
@@ -70,9 +70,23 @@ static int _accelerated(const vid_config_t *c, unsigned int sample_rate, unsigne
 		if(!t) return(0);
 		htv_tables_free(t);
 	}
+	if(c->s_video)
+	{
+		/* S-Video runs on the fused line kernels only: a chroma low-pass of fewer than 3 taps (PAL and NTSC at
+		 * 1.25 Msps and below), which the split modulators take, stays on the stock encoder */
+		htv_config_t hc;
+		htv_tables_t *t;
+		int ntaps = 0;
+		_translate(&hc, c);
+		t = htv_tables_create2(&hc, sample_rate, pixel_rate);
+		if(!t) return(0);
+		htv_tables_get(t, "chroma_taps", &ntaps);
+		htv_tables_free(t);
+		if(c->colour_mode != VID_SECAM && ntaps < 3) return(0);
+	}
 	if(c->videocrypt || c->videocrypt2 || c->videocrypts || c->syster ||
 	   c->d11 || c->systercnr || c->acp || c->sis || c->eurocrypt) return(0);
-	if(c->raw_bb_file || c->a2stereo || c->s_video || c->secam_field_id) return(0);
+	if(c->raw_bb_file || c->a2stereo || c->secam_field_id) return(0);
 	if(c->fm_left_level > 0 || c->fm_right_level > 0 || c->dance_level > 0) return(0);
 	if(c->interlace || c->frame_orientation) return(0);
 	return(1);
@@ -90,7 +104,7 @@ static void _translate(htv_config_t *h, const vid_config_t *c)
 	CP(gamma); CP(rw_co); CP(gw_co); CP(bw_co); CP(colour_mode); CP(volume); CP(colour_bw);
 	CP(burst_width); CP(burst_left); CP(burst_level); CP(burst_rise); CP(ev_co); CP(eu_co);
 	CP(fm_mono_carrier); CP(fm_mono_deviation); CP(fm_mono_preemph); CP(nicam_carrier); CP(nicam_beta);
-	CP(am_mono_carrier); CP(fm_level); CP(fm_deviation); CP(fm_energy_dispersal);
+	CP(am_mono_carrier); CP(fm_level); CP(fm_deviation); CP(fm_energy_dispersal); CP(s_video);
 #undef CP
 	h->frame_rate_num = c->frame_rate.num; h->frame_rate_den = c->frame_rate.den;
 	h->colour_carrier_num = c->colour_carrier.num; h->colour_carrier_den = c->colour_carrier.den;
