@@ -89,6 +89,24 @@ typedef struct {
 	uint64_t offset_phase0;        /* phase after the first renormalisation (see htv_tables.c) */
 } htv_dparams_t;
 
+#ifdef __CUDACC__
+#define HTV_HD __host__ __device__
+#else
+#define HTV_HD
+#endif
+
+/* The source picture row that line `line` (1 .. lines) of a frame shows, -1 none (ref video.c:2812-2895): a progressive
+ * source on an interlaced raster shifts down one row. The device's line_numbers and the host's picture-row table
+ * (htv_tables.c build_pic_rows) both take it from here. */
+static inline HTV_HD int htv_line_vy(const htv_dparams_t *dp, int line)
+{
+	int vy;
+	if(dp->raster == HTV_RASTER_625) vy = line < 313 ? (line - 23) * 2 : (line - 336) * 2 + 1;
+	else vy = line < 265 ? (line - 23) * 2 : (line - 286) * 2 + 1;
+	if(vy >= 0 && dp->interlaced != 0) vy += 1;
+	return(vy >= 0 && vy < dp->active_lines ? vy : -1);
+}
+
 /* Host-built tables (ref video.c:3812-4704, restated). All arrays are owned. */
 struct htv_tables_t {
 	htv_config_t conf;
@@ -99,6 +117,12 @@ struct htv_tables_t {
 	int16_t *pulse_values;  int npulse_values;
 	int16_t *tmpl_out, *tmpl_keep;                 /* [tmpl_rows][W] line templates: blank + sync pulses (htv_tables.c) */
 	uint8_t *tmpl_keep_any; int tmpl_rows;         /* lines + 2 */
+	/* rows of the converted picture store (htv_tables.c build_pic_rows): pic_rows[row] = line (1-based, 0: no line draws
+	 * the row), al, ar, keep of the line that shows it; rows 0 .. active_lines - 1 are the picture rows, the rest the
+	 * lines with a picture area and no source row (always black). line_row[line] = the row line `line` shows, -1: the
+	 * line has no picture area. */
+	int32_t *pic_rows;      int pic_nrows;
+	int32_t *line_row;
 	double glut[256];
 	htv_c16_t *clut;        size_t clut_len;      /* clut_width + W */
 	int16_t *burst_win;     int burst_width;

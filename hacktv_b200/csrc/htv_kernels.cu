@@ -55,7 +55,6 @@ struct DevGuard {
 
 struct DevTables {
 	const uint32_t *mma_atab;         // tap operand of the tensor-core video filter, fragment order (htv_mma_fir.h)
-	const uint32_t *chroma_atab;      // tap operand of the chroma low-pass for the fused line kernel: [hi, lo][lane] x 4 registers
 	const int16_t *tmpl_out, *tmpl_keep;   // line templates: blank + sync pulses (htv_tables.c build_templates)
 	const uint8_t *tmpl_keep_any;
 	const uint16_t *codes;
@@ -83,6 +82,13 @@ struct DevTables {
 	const int32_t *frame_map;         // slot of frame (first_frame + i)
 	int64_t frame_map_first;          // 0-based frame index of frame_map[0]
 	int32_t frame_map_len;
+	// converted picture store of the fused line kernel (k_picture): [slot][row][W], slot max_slots = black, row as
+	// htv_tables.c build_pic_rows; NULL on every other path
+	const int4 *pic_rows;             // [pic_nrows] line (1-based, 0 none), al, ar, keep of the line that shows the row
+	const int32_t *line_row;          // [lines + 1] the row line l shows, -1: no picture area
+	int32_t pic_nrows, pic_black;     // rows per slot; the black slot
+	int16_t *pic_val;                 // the line template outside [al, ar), Y + the template's keep part inside
+	uint32_t *pic_cuv;                // U | V << 16 after the chroma low-pass (colour encoders; NULL for mono)
 	// audio state rings
 	const int16_t *pcm;               // RA stereo pairs, index j & (RA-1)
 	int32_t *lim_var, *lim_fix;       // RA, index j & (RA-1)
@@ -206,6 +212,8 @@ struct htv_dev_t {
 	cudaEvent_t ev_nic;
 	cudaStream_t up;                  // picture / PCM uploads: ahead of the previous chunk's kernels
 	cudaEvent_t ev_up, ev_chunk[2];
+	cudaStream_t pic;                 // the converted picture store (k_picture), behind each picture's copy but off the
+	cudaEvent_t ev_copied, ev_pic;    // upload stream, so that the next copies do not queue behind the conversions
 	unsigned chunk_i;
 	cudaEvent_t ev_in, ev_audio;
 	cudaEvent_t ev_kl[2];             // the fused line kernel has read descriptor buffer 0 / 1
@@ -640,7 +648,8 @@ struct __align__(16) LineR2 {
 	unsigned int clut_off;
 	int ov_to, ov_value, ov_add;      // ov_add: row of dt.ov_add, -1 none; ov_from >= ov_to: no replace
 	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
-	long long pad;
+	long long pic;                    // k_line: offset of the line's row in the converted picture store (dt.pic_val,
+	                                  // dt.pic_cuv), -1: no picture area, the template row is the line
 };
 static_assert(sizeof(LineR2) == 64, "LineR2 is read as four int4");
 
@@ -663,6 +672,13 @@ static_assert(sizeof(LineS2) == 64, "LineS2 is read as four int4");
 
 static_assert(sizeof(LineA2) % 16 == 0, "descriptors are copied as int4");
 
+// the picture slot of 0-based frame f0, -1: the source has no picture (black)
+__device__ __forceinline__ int frame_slot(const DevTables &dt, int64_t f0)
+{
+	const int64_t fi = f0 - dt.frame_map_first;
+	return(fi >= 0 && fi < dt.frame_map_len ? dt.frame_map[fi] : -1);
+}
+
 // frame / line / picture row of scan line L; L < 0 are the pipeline-fill lines the reference's
 // SECAM stage sees before line 1 (frame 1, line 0: an all-black active line, ref video.c:4665-4667)
 __device__ __forceinline__ void line_numbers(const htv_dparams_t &dp, const DevTables &dt, int64_t L,
@@ -674,20 +690,11 @@ __device__ __forceinline__ void line_numbers(const htv_dparams_t &dp, const DevT
 	frame = (int) (f0 + 1);
 	line = (int) (L - f0 * dp.lines) + 1;
 	code = dt.codes[line];
-	// source row (ref video.c:2812-2895): a progressive source on an interlaced raster shifts down one row
-	int vy;
-	if(dp.raster == HTV_RASTER_625) vy = line < 313 ? (line - 23) * 2 : (line - 336) * 2 + 1;
-	else vy = line < 265 ? (line - 23) * 2 : (line - 286) * 2 + 1;
-	if(vy >= 0 && dp.interlaced != 0) vy += 1;
-	if(vy < 0 || vy >= dp.active_lines) vy = -1;
+	const int vy = htv_line_vy(&dp, line);
 	if(vy >= 0 && dt.frames)
 	{
-		const int64_t fi = f0 - dt.frame_map_first;
-		if(fi >= 0 && fi < dt.frame_map_len)
-		{
-			const int slot = dt.frame_map[fi];              // -1: the source has no picture (black)
-			if(slot >= 0) row_off = ((long long) slot * dp.active_lines + vy) * (long long) dp.active_width;
-		}
+		const int slot = frame_slot(dt, f0);
+		if(slot >= 0) row_off = ((long long) slot * dp.active_lines + vy) * (long long) dp.active_width;
 	}
 }
 
@@ -771,7 +778,14 @@ __global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const De
 	o.ov_any = line_overlay(dt, L, m);
 	o.ov_from = m.x; o.ov_to = m.y; o.ov_value = m.z; o.ov_add = m.w;
 	o.row_off = row_off;
-	o.pad = 0;
+	// the converted row: of the frame's picture, of the black slot where the frame has none or the line no source row
+	o.pic = -1;
+	if(dt.pic_val && al < ar)
+	{
+		const int row = dt.line_row[line];
+		const int slot = row < dp.active_lines ? frame_slot(dt, frame - 1) : -1;
+		o.pic = ((long long) (slot >= 0 ? slot : dt.pic_black) * dt.pic_nrows + row) * dp.W;
+	}
 	reinterpret_cast<LineR2 *>(out)[i] = o;
 }
 
@@ -1175,6 +1189,47 @@ __device__ __forceinline__ void store_line4(const int (&val)[SPT], int x0, int W
 	}
 }
 
+// A thread's line values x0 .. x0 + 3 before the subcarrier (ref video.c:2864-2992): row `tmpl` of the line templates
+// outside the picture area [al, ar), the picture's Y plus the template's keep part inside it; U, V inside it, 0 outside.
+// rgb: the source row (pixel x at rgb[x - active_left]), NULL: black. k_raster and k_picture raster through here.
+__device__ __forceinline__ void raster_pic4(const htv_dparams_t &dp, const DevTables &dt, int tmpl, int al, int ar, bool keep,
+	const uint32_t *rgb, int x0, int (&val)[SPT], int (&uu)[SPT], int (&vv)[SPT])
+{
+	const int W = dp.W, trow = tmpl * W;
+	#pragma unroll
+	for(int k = 0; k < SPT; k++)
+	{
+		const int x = x0 + k;
+		val[k] = x < W ? __ldg(dt.tmpl_out + trow + x) : 0; uu[k] = 0; vv[k] = 0;
+		if(x >= al && x < ar)
+		{
+			yuv_lookup(dt, rgb ? (__ldg(rgb + (x - dp.active_left)) & 0xFFFFFF) : 0, val[k], uu[k], vv[k]);
+			if(keep) val[k] += __ldg(dt.tmpl_keep + trow + x);           // the next line's leading edge
+		}
+	}
+}
+
+// The chroma low-pass of samples x0 .. x0 + 3 from the U, V windows su, sv (index x + UOFF, zero outside the picture)
+__device__ __forceinline__ void chroma_lp4(const htv_dparams_t &dp, const int *su, const int *sv, int x0, int (&cu)[SPT], int (&cv)[SPT])
+{
+	// every tap count a raster up to the kernels' 1536-sample width has (7 at 9 MHz, 17 at 24 MHz); the lower ones only
+	// the --pixelrate raster and the split path run
+	switch(dp.chroma_ntaps)
+	{
+	case 1: chroma_fir4<1>(dp, su, sv, x0, cu, cv); break;
+	case 3: chroma_fir4<3>(dp, su, sv, x0, cu, cv); break;
+	case 5: chroma_fir4<5>(dp, su, sv, x0, cu, cv); break;
+	case 7: chroma_fir4<7>(dp, su, sv, x0, cu, cv); break;
+	case 9: chroma_fir4<9>(dp, su, sv, x0, cu, cv); break;
+	case 11: chroma_fir4<11>(dp, su, sv, x0, cu, cv); break;
+	case 13: chroma_fir4<13>(dp, su, sv, x0, cu, cv); break;
+	case 15: chroma_fir4<15>(dp, su, sv, x0, cu, cv); break;
+	case 17: chroma_fir4<17>(dp, su, sv, x0, cu, cv); break;
+	default:                                                            // no chroma low-pass (chroma_ntaps = 0)
+		for(int k = 0; k < SPT; k++) { cu[k] = su[x0 + k + UOFF]; cv[k] = sv[x0 + k + UOFF]; }
+	}
+}
+
 // ---------------------------------------------------------------------------
 // Raster kernel: one CTA per scan line, 4 samples per thread -> int16 composite stream
 // (ref video.c:2864-3066 _vid_next_line_raster, vbidata.c:186-239). Low register count
@@ -1210,21 +1265,8 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 	if(x0 < W)
 	{
 		// ---- blanking and sync from the line template, luma, unfiltered U,V ------
-		const int trow = li.tmpl * W;
 		int uu[SPT], vv[SPT];
-		#pragma unroll
-		for(int k = 0; k < SPT; k++)
-		{
-			const int x = x0 + k;
-			val[k] = x < W ? __ldg(dt.tmpl_out + trow + x) : 0; uu[k] = 0; vv[k] = 0;
-			if(x >= li.al && x < li.ar)
-			{
-				const unsigned int rgb = li.row_off >= 0 ? (__ldg(dt.frames + li.row_off + (x - dp.active_left)) & 0xFFFFFF) : 0;
-				yuv_lookup(dt, rgb, val[k], uu[k], vv[k]);
-				if(li.keep) val[k] += __ldg(dt.tmpl_keep + trow + x);       // the next line's leading edge
-				if(!li.pal) uu[k] = vv[k] = 0;
-			}
-		}
+		raster_pic4(dp, dt, li.tmpl, li.al, li.ar, li.keep, li.row_off >= 0 ? dt.frames + li.row_off : NULL, x0, val, uu, vv);
 		if(li.pal)
 		{
 			*reinterpret_cast<int4 *>(su + x0 + UOFF) = make_int4(uu[0], uu[1], uu[2], uu[3]);
@@ -1243,25 +1285,7 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 			if(near_pic || near_burst)
 			{
 				int cu[SPT] = { 0, 0, 0, 0 }, cv[SPT] = { 0, 0, 0, 0 };
-				if(near_pic)
-				{
-					// every tap count a raster up to the kernels' 1536-sample width has (7 at 9 MHz, 17 at 24 MHz); the
-					// lower ones only the --pixelrate raster and the split path run
-					switch(dp.chroma_ntaps)
-					{
-					case 1: chroma_fir4<1>(dp, su, sv, x0, cu, cv); break;
-					case 3: chroma_fir4<3>(dp, su, sv, x0, cu, cv); break;
-					case 5: chroma_fir4<5>(dp, su, sv, x0, cu, cv); break;
-					case 7: chroma_fir4<7>(dp, su, sv, x0, cu, cv); break;
-					case 9: chroma_fir4<9>(dp, su, sv, x0, cu, cv); break;
-					case 11: chroma_fir4<11>(dp, su, sv, x0, cu, cv); break;
-					case 13: chroma_fir4<13>(dp, su, sv, x0, cu, cv); break;
-					case 15: chroma_fir4<15>(dp, su, sv, x0, cu, cv); break;
-					case 17: chroma_fir4<17>(dp, su, sv, x0, cu, cv); break;
-					default:                                        // no chroma low-pass (chroma_ntaps = 0)
-						for(int k = 0; k < SPT; k++) { cu[k] = su[x0 + k + UOFF]; cv[k] = sv[x0 + k + UOFF]; }
-					}
-				}
+				if(near_pic) chroma_lp4(dp, su, sv, x0, cu, cv);
 				#pragma unroll
 				for(int k = 0; k < SPT; k++)
 				{
@@ -1292,6 +1316,57 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 		}
 	}
 	store_line4(val, x0, W, comp, comp32, planes, plane_stride, plane_pitch);
+}
+
+// ---------------------------------------------------------------------------
+// Converted picture store of the fused line kernel: the part of a line that depends on the picture and on the line's
+// place in the frame only - the line template, Y, and U / V through the chroma low-pass - converted once per picture
+// when it arrives (htv_dev_upload_frame[s]), not on every line that shows it. One CTA per row `blockIdx.x` of picture
+// slot `slot0 + blockIdx.y` (slot max_slots, the black slot: from zero RGB), 4 samples per thread, as k_raster's first
+// half; the line of the row and its geometry come from the host (htv_tables.c build_pic_rows). What k_line takes from
+// here is what k_raster computes up to the burst: dt.pic_val = val[], dt.pic_cuv = (cu, cv) over the whole line.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(384)
+k_picture(const __grid_constant__ htv_dparams_t dp, const DevTables dt, int slot0)
+{
+	extern __shared__ __align__(16) unsigned char smem_raw[];
+	const int W = dp.W, W4 = (W + 3) & ~3;
+	int *su = reinterpret_cast<int *>(smem_raw);                    // index = x + UOFF
+	int *sv = su + W4 + 2 * UOFF;
+	const int tid = threadIdx.x, row = blockIdx.x, slot = slot0 + blockIdx.y;
+	const int4 g = __ldg(dt.pic_rows + row);                        // line, al, ar, keep
+	if(g.x == 0) return;                                            // no line shows this row
+	const bool black = slot == dt.pic_black;
+	if(tid < 2 * UOFF)
+	{
+		const int j = tid < UOFF ? tid : W4 + tid;
+		su[j] = 0; sv[j] = 0;
+	}
+	const int x0 = tid * SPT;
+	const size_t at = ((size_t) slot * dt.pic_nrows + row) * W + x0;
+	int val[SPT], uu[SPT], vv[SPT];
+	if(x0 < W)
+	{
+		const uint32_t *rgb = black ? NULL : dt.frames + ((size_t) slot * dp.active_lines + row) * dp.active_width;
+		raster_pic4(dp, dt, g.x - 1, g.y, g.z, g.w, rgb, x0, val, uu, vv);
+		#pragma unroll
+		if((W & 3) == 0)                                            // at is a multiple of 4: one 8-byte store
+			*reinterpret_cast<uint2 *>(dt.pic_val + at) = make_uint2((val[0] & 0xFFFF) | (val[1] << 16), (val[2] & 0xFFFF) | (val[3] << 16));
+		else for(int k = 0; k < SPT; k++) if(x0 + k < W) dt.pic_val[at + k] = (int16_t) val[k];
+		*reinterpret_cast<int4 *>(su + x0 + UOFF) = make_int4(uu[0], uu[1], uu[2], uu[3]);
+		*reinterpret_cast<int4 *>(sv + x0 + UOFF) = make_int4(vv[0], vv[1], vv[2], vv[3]);
+	}
+	if(!dt.pic_cuv) return;
+	__syncthreads();
+	if(x0 >= W) return;
+	int cu[SPT], cv[SPT];
+	chroma_lp4(dp, su, sv, x0, cu, cv);
+	#pragma unroll
+	unsigned w[SPT];
+	#pragma unroll
+	for(int k = 0; k < SPT; k++) w[k] = ((unsigned) cu[k] & 0xFFFFu) | ((unsigned) cv[k] << 16);
+	if((W & 3) == 0) *reinterpret_cast<uint4 *>(dt.pic_cuv + at) = make_uint4(w[0], w[1], w[2], w[3]);
+	else for(int k = 0; k < SPT; k++) if(x0 + k < W) dt.pic_cuv[at + k] = w[k];
 }
 
 // ---------------------------------------------------------------------------
@@ -2417,7 +2492,9 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	{
 		// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768. The Gaussian taps are
 		// rounded one by one, so at about 1 % of sample rates they sum to 32769 .. 32771 (17.734475, 20.05 Msps: 32769),
-		// and those rates run the CSAT form
+		// and those rates run the CSAT form. The saturation itself is k_picture's now, so the CSAT forms run the code of
+		// the partial-tile form; they, and the partial-tile form for CSAT rates where 128 divides W, stay only because the
+		// instantiation names htv_line_kernel reports are pinned by the tests
 		long long sum = 0;
 		for(int i = 0; i < dp.chroma_ntaps; i++) sum += dp.chroma_taps[i] < 0 ? -dp.chroma_taps[i] : dp.chroma_taps[i];
 		const int csat = sum > 32768;
@@ -2482,7 +2559,7 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	if(p->kl)
 	{
 		kl_name(kl, sizeof(kl), *p->kl, type, dp.s_video);
-		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 6 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + 4 * uvb + 1024 + ntp + 128;
+		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
 		// S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
 		if(dp.s_video && p->path == PATH_LINE) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
 	}
@@ -2529,11 +2606,12 @@ extern "C" int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, 
 
 // An encoder's side streams and events, in the one list htv_dev_create creates and htv_dev_destroy destroys. ev0 and
 // ev1 time the last modulator launch (htv_dev_last_line_ms); every other event only orders work, without timing.
-struct DevSync { cudaStream_t *stream[4]; cudaEvent_t *timed[2]; cudaEvent_t *event[9]; };
+struct DevSync { cudaStream_t *stream[5]; cudaEvent_t *timed[2]; cudaEvent_t *event[11]; };
 static DevSync dev_sync(htv_dev_t *d)
 {
-	return(DevSync{ { &d->side, &d->side2, &d->side3, &d->up }, { &d->ev0, &d->ev1 },
-		{ &d->ev_nic, &d->ev_up, &d->ev_chunk[0], &d->ev_chunk[1], &d->ev_in, &d->ev_kl[0], &d->ev_kl[1], &d->ev_r2, &d->ev_audio } });
+	return(DevSync{ { &d->side, &d->side2, &d->side3, &d->up, &d->pic }, { &d->ev0, &d->ev1 },
+		{ &d->ev_nic, &d->ev_up, &d->ev_chunk[0], &d->ev_chunk[1], &d->ev_in, &d->ev_kl[0], &d->ev_kl[1], &d->ev_r2, &d->ev_audio,
+		  &d->ev_copied, &d->ev_pic } });
 }
 
 // htv_dev_create's way out: the message, and everything allocated so far freed
@@ -2616,6 +2694,19 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	d->d_pcm = (int16_t *) dev_zero(d, sizeof(int16_t) * 2 * RA);
 	dt.frames = d->d_frames;
 	dt.frame_map = d->d_frame_map;
+	if(p.path == PATH_LINE)
+	{
+		// the converted picture store (k_picture): a row per source row of every slot and of the black slot, which also
+		// holds the lines with a picture area and no source row; (max_slots + 1) x pic_nrows x W x 6 bytes (60 MB for
+		// PAL at 16 Msps)
+		dt.pic_rows = (const int4 *) dev_copy(d, t->pic_rows, sizeof(int32_t) * 4 * t->pic_nrows);
+		dt.line_row = (const int32_t *) dev_copy(d, t->line_row, sizeof(int32_t) * (dp.lines + 1));
+		dt.pic_nrows = t->pic_nrows;
+		dt.pic_black = d->max_slots;
+		const size_t n = (size_t) (d->max_slots + 1) * t->pic_nrows * dp.W;
+		dt.pic_val = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
+		if(dp.colour_mode != HTV_MONOCHROME) dt.pic_cuv = (uint32_t *) dev_zero(d, sizeof(uint32_t) * n);
+	}
 	dt.pcm = d->d_pcm;
 	if(dp.have_fm)
 	{
@@ -2698,13 +2789,12 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 			nt[((s3 * 2 + lo) * 32 + lane) * 4 + reg] = mf_a_word(dp.secam_notch, s3, lane, reg, lo);
 		dt.notch_atab = (const uint32_t *) dev_copy(d, nt, sizeof(nt));
 	}
-	auto lp_atab = [d](const int32_t *taps, int ntaps) {                 // a low-pass of one k-step: the chroma's, SECAM's baseband
+	auto lp_atab = [d](const int32_t *taps, int ntaps) {                 // a low-pass of one k-step: SECAM's baseband
 		uint32_t ctab[256];
 		for(int lo = 0; lo < 2; lo++) for(int lane = 0; lane < 32; lane++) for(int reg = 0; reg < 4; reg++)
 			ctab[(lo * 32 + lane) * 4 + reg] = kl_chroma_a_word(taps, ntaps, lane, reg, lo);
 		return((const uint32_t *) dev_copy(d, ctab, sizeof(ctab)));
 	};
-	if(p.path == PATH_LINE && dp.colour_mode != HTV_MONOCHROME) dt.chroma_atab = lp_atab(dp.chroma_taps, dp.chroma_ntaps);
 	if(p.ks) dt.sec_lpf_atab = lp_atab(dp.secam_lpf, 15);
 	if(secam)
 	{
@@ -2737,6 +2827,8 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	}
 	if(d->alloc_failed) return(create_fail(d, err, errlen, "device allocation failed"));
 	if(!plan_attributes(p, err, errlen)) { htv_dev_destroy(d); return(NULL); }
+	// the black slot, once: every row from zero RGB, behind the RGB -> YUV table on the default stream
+	if(dt.pic_val) k_picture<<<dim3(dt.pic_nrows, 1), p.line_threads, p.raster_smem>>>(dp, dt, dt.pic_black);
 	const DevSync sy = dev_sync(d);
 	bool made = true;
 	for(cudaStream_t *s : sy.stream) made &= cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
@@ -2785,6 +2877,11 @@ extern "C" int htv_dev_uploads_end(htv_dev_t *d, void *stream)
 	DevGuard guard(d->device);
 	CK(cudaEventRecord(d->ev_up, d->up));
 	CK(cudaStreamWaitEvent((cudaStream_t) stream, d->ev_up, 0));
+	if(d->dt.pic_val)
+	{
+		CK(cudaEventRecord(d->ev_pic, d->pic));
+		CK(cudaStreamWaitEvent((cudaStream_t) stream, d->ev_pic, 0));
+	}
 	return(HTV_OK);
 }
 
@@ -2831,13 +2928,30 @@ extern "C" int htv_dev_set_overlays(htv_dev_t *d, int n, const long long *line, 
 	return(HTV_OK);
 }
 
+// The converted picture store of slots slot .. slot + count - 1, right behind their copy on `st` (fused line kernel only).
+// Its slots are under the RGB slots' protection: the host cycles 16 slots and brings at most 7 new pictures per call
+// (htv_host.c), and the uploads of call c wait for call c - 2's kernels (htv_dev_uploads_begin), which the conversion
+// waits for through its copy. It runs on a stream of its own, so that the next copies on the upload stream go on
+// beside it; htv_dev_uploads_end makes the caller's stream wait for it (ev_pic) as for the copies (ev_up). Call c + 1's
+// copies touch none of the RGB slots call c converts: they are the next 7 of the 16.
+static int convert_pictures(htv_dev_t *d, int slot, int count, cudaStream_t st)
+{
+	if(!d->dt.pic_val) return(HTV_OK);
+	CK(cudaEventRecord(d->ev_copied, st));
+	CK(cudaStreamWaitEvent(d->pic, d->ev_copied, 0));
+	k_picture<<<dim3(d->dp.active_lines, count), d->plan.line_threads, d->plan.raster_smem, d->pic>>>(d->dp, d->dt, slot);
+	d->launches++;
+	CK(cudaGetLastError());
+	return(HTV_OK);
+}
+
 extern "C" int htv_dev_upload_frame(htv_dev_t *d, int slot, const uint32_t *rgb, void *stream)
 {
 	DevGuard guard(d->device);
 	if(slot < 0 || slot >= d->max_slots) return(HTV_ERROR);
 	CK(cudaMemcpyAsync(d->d_frames + (size_t) slot * d->frame_pixels, rgb, d->frame_pixels * 4,
 		cudaMemcpyHostToDevice, (cudaStream_t) stream));
-	return(HTV_OK);
+	return(convert_pictures(d, slot, 1, (cudaStream_t) stream));
 }
 
 // `count` pictures, contiguous in host memory, into `count` consecutive slots: one copy
@@ -2845,8 +2959,16 @@ extern "C" int htv_dev_upload_frames(htv_dev_t *d, int slot, int count, const ui
 {
 	DevGuard guard(d->device);
 	if(slot < 0 || count < 1 || slot + count > d->max_slots) return(HTV_ERROR);
-	CK(cudaMemcpyAsync(d->d_frames + (size_t) slot * d->frame_pixels, rgb, d->frame_pixels * 4 * (size_t) count,
-		cudaMemcpyHostToDevice, (cudaStream_t) stream));
+	// with the picture store, the last picture goes up in a copy of its own: the others are converted while it is copied,
+	// so that one picture's conversion, not the run's, stands between the copies and the line kernel that waits for both
+	const int head = d->dt.pic_val && count > 1 ? count - 1 : count;
+	for(int at = 0, n = head; at < count; at += n, n = count - at)
+	{
+		CK(cudaMemcpyAsync(d->d_frames + (size_t) (slot + at) * d->frame_pixels, rgb + (size_t) at * d->frame_pixels,
+			d->frame_pixels * 4 * (size_t) n, cudaMemcpyHostToDevice, (cudaStream_t) stream));
+		const int r = convert_pictures(d, slot + at, n, (cudaStream_t) stream);
+		if(r != HTV_OK) return(r);
+	}
 	return(HTV_OK);
 }
 

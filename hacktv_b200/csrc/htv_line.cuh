@@ -4,9 +4,10 @@
 // the picture in HBM and the int16 IQ in HBM - raster, chroma, video filter, sound carriers, mixers -
 // without the composite signal ever leaving the SM:
 //
-//   R1  template (blank + sync pulses) + picture: RGB -> Y,U,V by table (ref video.c:2864-2992)
-//   R2  chroma low-pass on the tensor cores, burst, subcarrier mix (ref video.c:3011-3040, fir.c:357-375),
-//       VBI overlay; the finished composite line goes into a 3-row ring of byte planes in shared memory
+//   R1  the line's row of the converted picture store: template (blank + sync pulses) + Y, and U, V after the chroma
+//       low-pass, converted once per picture when it arrived (k_picture, ref video.c:2864-2992, fir.c:357-375)
+//   R2  burst, subcarrier mix (ref video.c:3011-3040), VBI overlay; the finished composite line goes into a 4-row ring
+//       of byte planes in shared memory
 //   M   51-tap VSB / low-pass video filter on the tensor cores (ref video.c:3235-3248, fir.c:564-615),
 //       FM / AM / NICAM sound carriers (ref video.c:3261-3450, nicam728.c:342-411), IQ swap, offset
 //       mixer (ref video.c:3466-3515), channel combiner, store.
@@ -98,18 +99,21 @@ __device__ __forceinline__ void kl_cp16(void *dst_smem, const void *src)
 __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // VF: a video filter is on (composite ring + tensor-core FIR); HASQ: it has Q taps (VSB); FULL: 128 | W (no
-// partial tile: the x < W tests fold away); CSAT: the chroma low-pass can leave the int16 range (sum of |taps| > 32768)
+// partial tile: the x < W tests fold away); CSAT: the chroma low-pass can leave the int16 range (sum of |taps| > 32768),
+// which k_picture's saturating low-pass handles when it fills the store: the CSAT forms run the same code as the others
 //
 // Per iteration q (one scan line) a CTA runs
-//   R1b(q)  picture values by table from the pixels fetched earlier, U / V byte planes        | __syncthreads (colour lines)
-//   R2(q)   chroma low-pass (mma), burst, subcarrier, VBI overlay, composite row q mod 3       | __syncthreads
-//   R1a(q+1) template + pixel loads of the NEXT line are issued here ...
+//   R2(q)   burst, subcarrier, VBI overlay on the values fetched earlier, composite row q mod 4  | __syncthreads
+//   R1(q+1) the converted row of the NEXT line (values, and filtered U / V on colour lines) is loaded here ...
 //   M(q-1)  ... and arrive while line q - 1 (whose right-hand halo R2(q) has just written) is filtered (mma),
 //           gets its sound carriers and is stored.
 // The line descriptors (LineR2 of q + 1, LineA2 of q - 1) come in by cp.async at the top of the iteration.
+// One barrier per line, so the ring has 4 rows: a warp that is through M(q - 1) may run on into R2(q + 1), before the
+// next barrier, while another warp is still reading line q - 1's row. R2(q + 1) writes line q + 1's row, the right
+// halo of line q's and the left halo of line q + 2's; with 4 rows none of them is line q - 1's.
 //
 // SRC: the composite lines are not rastered here but read from `src` (row q + 2 = relative line q, int16): SECAM, whose
-// chrominance chain (htv_secam.cuh) runs between the raster and the modulator. R1b / R2 fold away, the rest is the same.
+// chrominance chain (htv_secam.cuh) runs between the raster and the modulator. R2 folds away, the rest is the same.
 // WC: the line width compiled in (0: dp.W), so that the shared-memory row and plane offsets become immediates
 // ST: the output sample type compiled into the store (HTV_TYPE_INT16: the int16 store), -1: dp.sample_type at run time
 //
@@ -124,16 +128,13 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = WC ? WC : dp.W;
-	const int RB = kl_row_bytes(W), UB = kl_uv_bytes(W);
-	// descriptors x2 | [row 0..2][hi, lo] composite planes | [u hi, u lo, v hi, v lo] | FIR taps | chroma taps | NICAM pulse |
-	// S-Video chroma [row 0..1][j][thread]
+	const int RB = kl_row_bytes(W);
+	// descriptors x2 | [row 0..3][hi, lo] composite planes | FIR taps | NICAM pulse | S-Video chroma [row 0..1][j][thread]
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
 	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + 2);
 	unsigned char *rows = reinterpret_cast<unsigned char *>(slr + 2);
-	unsigned char *uvp = rows + (VF ? 6 * RB : 0);
-	uint4 *atab = reinterpret_cast<uint4 *>(uvp + 4 * UB);                 // [k-step][I hi, I lo, Q hi, Q lo][lane]
-	uint4 *ctab = atab + (VF ? MF_ATAB_WORDS / 4 : 0);                      // [hi, lo][lane]
-	short *ntp = reinterpret_cast<short *>(ctab + 64);
+	uint4 *atab = reinterpret_cast<uint4 *>(rows + (VF ? 8 * RB : 0));    // [k-step][I hi, I lo, Q hi, Q lo][lane]
+	short *ntp = reinterpret_cast<short *>(atab + (VF ? MF_ATAB_WORDS / 4 : 0));
 	const int tid = threadIdx.x, lane = tid & 31, nt = tid >> 5;
 	const int g = lane >> 2, t = lane & 3;
 	const int xb = mf_lane_x(nt, lane, 0);                                  // the lane's samples: xb + 8 j
@@ -147,8 +148,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 
 	// ---- one-time set-up -------------------------------------------------------
 	if(VF) for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
-	if(dt.chroma_atab) for(int i = tid; i < 64; i += blockDim.x) ctab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.chroma_atab) + i);
-	for(int i = tid; i < ((VF ? 6 * RB : 0) + 4 * UB) / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
+	if(VF) for(int i = tid; i < 8 * RB / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
 	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
 	{
 		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
@@ -158,19 +158,16 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	if(!SRC && tid < 4) reinterpret_cast<int4 *>(slr + (q0 & 1))[tid] = __ldg(reinterpret_cast<const int4 *>(lrp + q0 + 1) + tid);
 	__syncthreads();
 
-	const int full_l = dp.active_left, full_r = dp.active_left + dp.active_width;
-	const bool in_full = xb + 24 >= full_l && xb < full_r;                  // the lane touches the picture area at all
-	const bool all_full = xb >= full_l && xb + 24 < full_r;                 // ... with all four samples
+	// the span the chroma low-pass reaches (taps <= 17: 8 samples either side of the picture); the store is zero outside
+	const bool in_chroma = xb + 24 >= dp.active_left - 8 && xb < dp.active_left + dp.active_width + 8;
 	const bool in_burst = xb + 24 >= dp.burst_left && xb < dp.burst_left + dp.burst_width;
-	unsigned char *const uv0 = uvp + KL_UVLEAD + xb;                        // the lane's bytes in the four chroma planes
-	const unsigned char *const uvb = uvp + mf_lp_b_offset(nt, lane);        // ... and its chroma B fragment
 	const int fo0 = mf_b_offset(nt, 0, lane);
 	constexpr int NA16 = (int) (sizeof(LineA2) / 16);
 
-	// loads of line q issued one phase early: template (int16 x 4) and pixels (RGBx x 4)
+	// loads of line q issued one phase early: line values (int16 x 4) and, on colour lines, filtered U | V << 16 (x 4)
 	int tm[4];
 	unsigned px[4];
-	#define KL_R1A(QQ) do { \
+	#define KL_R1(QQ) do { \
 		if(SRC) \
 		{ \
 			const int16_t *sp_ = src + (size_t) ((QQ) + 2) * W + xb; \
@@ -179,117 +176,42 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			break; \
 		} \
 		const LineR2 &ln = slr[(QQ) & 1]; \
-		const int16_t *tp_ = dt.tmpl_out + (size_t) ln.tmpl * W + xb; \
+		const long long pic_ = ln.pic; \
+		const int16_t *tp_ = (pic_ >= 0 ? dt.pic_val + pic_ : dt.tmpl_out + (size_t) ln.tmpl * W) + xb; \
 		_Pragma("unroll") for(int j = 0; j < 4; j++) tm[j] = (FULL || xb + 8 * j < W) ? (int) __ldg(tp_ + 8 * j) : 0; \
-		if(in_full && ln.al < ln.ar && ln.row_off >= 0) \
+		if(in_chroma && ln.pal && pic_ >= 0) \
 		{ \
-			const uint32_t *pp_ = dt.frames + ln.row_off + (xb - dp.active_left); \
-			_Pragma("unroll") for(int j = 0; j < 4; j++) \
-			{ \
-				const int x_ = xb + 8 * j; \
-				px[j] = (x_ >= ln.al && x_ < ln.ar) ? __ldg(pp_ + 8 * j) : 0u; \
-			} \
+			const uint32_t *cp_ = dt.pic_cuv + pic_ + xb; \
+			_Pragma("unroll") for(int j = 0; j < 4; j++) px[j] = (FULL || xb + 8 * j < W) ? __ldg(cp_ + 8 * j) : 0u; \
 		} \
 		else { px[0] = px[1] = px[2] = px[3] = 0u; } \
 	} while(0)
-	KL_R1A(q0);
+	KL_R1(q0);
 
-	int r3 = (q0 + 3) % 3;                                                  // ring row of line q
-	for(int q = q0; q <= q1; q++, r3 = r3 == 2 ? 0 : r3 + 1)
+	int r4 = q0 & 3;                                                        // ring row of line q
+	for(int q = q0; q <= q1; q++, r4 = (r4 + 1) & 3)
 	{
 		const int mrow = VF ? q - 1 : q;                                    // the line modulated in this iteration
 		// ---- descriptors of the next raster line and of the line modulated below -> shared memory -----
 		if(tid < 4) { if(!SRC && q + 1 <= q1) kl_cp16(reinterpret_cast<int4 *>(slr + ((q + 1) & 1)) + tid, reinterpret_cast<const int4 *>(lrp + q + 2) + tid); }
 		else if(tid < 4 + NA16) { if(mrow >= a) kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + (tid - 4), reinterpret_cast<const int4 *>(lap + mrow) + (tid - 4)); }
 
-		// ---- R1b: picture values of line q ---------------------------------------
+		// ---- R2: burst, subcarrier, VBI overlay of line q ---------------------------
 		const LineR2 &li = slr[q & 1];
-		const int li_al = SRC ? 0 : li.al, li_ar = SRC ? 0 : li.ar, li_pal = SRC ? 0 : li.pal;
+		const int li_pal = SRC ? 0 : li.pal;
 		int val[4] = { tm[0], tm[1], tm[2], tm[3] };
-		int uu[4] = { 0, 0, 0, 0 }, vv[4] = { 0, 0, 0, 0 };
 		int cq[4] = { 0, 0, 0, 0 };                                         // S-Video: the chroma of line q
-		if(in_full && li_al < li_ar)
-		{
-			if(xb >= li_al && xb + 24 < li_ar && !li.keep)
-			{
-				// all four samples in the picture
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					const short4 e = __ldg(dt.yuv_lut + (px[j] & 0xFFFFFFu));
-					val[j] = e.x; uu[j] = e.y; vv[j] = e.z;
-				}
-			}
-			else
-			{
-				const int16_t *kp = dt.tmpl_keep + (size_t) li.tmpl * W + xb;
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					const int x = xb + 8 * j;
-					if(x >= li_al && x < li_ar)
-					{
-						const short4 e = __ldg(dt.yuv_lut + (px[j] & 0xFFFFFFu));
-						val[j] = e.x; uu[j] = e.y; vv[j] = e.z;
-						if(li.keep) val[j] += __ldg(kp + 8 * j);
-					}
-				}
-			}
-		}
 		if(li_pal)
 		{
-			// subcarrier table entries of this line: in flight across the barrier and the chroma filter
 			short2 cl[4];
 			{
 				const htv_c16_t *cp = dt.clut + li.clut_off + xb;
 				#pragma unroll
 				for(int j = 0; j < 4; j++) cl[j] = (FULL || xb + 8 * j < W) ? kl_ldc16(cp + 8 * j) : make_short2(0, 0);
 			}
-			// unfiltered U, V as byte planes; outside the picture the planes stay zero (the reference filters
-			// each line on its own: zero history either side, ref fir.c:357-375)
-			if(all_full)
-			{
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					uv0[8 * j] = (unsigned char) (uu[j] >> 8); uv0[UB + 8 * j] = (unsigned char) uu[j];
-					uv0[2 * UB + 8 * j] = (unsigned char) (vv[j] >> 8); uv0[3 * UB + 8 * j] = (unsigned char) vv[j];
-				}
-			}
-			else if(in_full)
-			{
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					const int x = xb + 8 * j;
-					if(x >= full_l && x < full_r)
-					{
-						uv0[8 * j] = (unsigned char) (uu[j] >> 8); uv0[UB + 8 * j] = (unsigned char) uu[j];
-						uv0[2 * UB + 8 * j] = (unsigned char) (vv[j] >> 8); uv0[3 * UB + 8 * j] = (unsigned char) vv[j];
-					}
-				}
-			}
-			__syncthreads();
-			// ---- R2: chroma low-pass (tensor cores), burst, subcarrier ---------------
 			int cu[4], cv[4];
-			{
-				int uhh[4] = { 0, 0, 0, 0 }, umid[4] = { 0, 0, 0, 0 }, ull[4] = { 0, 0, 0, 0 };
-				int vhh[4] = { 0, 0, 0, 0 }, vmid[4] = { 0, 0, 0, 0 }, vll[4] = { 0, 0, 0, 0 };
-				const uint4 ah = ctab[lane], al4 = ctab[32 + lane];
-				const uint2 uh = *reinterpret_cast<const uint2 *>(uvb), ul = *reinterpret_cast<const uint2 *>(uvb + UB);
-				const uint2 vh = *reinterpret_cast<const uint2 *>(uvb + 2 * UB), vl = *reinterpret_cast<const uint2 *>(uvb + 3 * UB);
-				mma_ss(uhh, ah, uh); mma_su(umid, ah, ul); mma_us(umid, al4, uh); mma_uu(ull, al4, ul);
-				mma_ss(vhh, ah, vh); mma_su(vmid, ah, vl); mma_us(vmid, al4, vh); mma_uu(vll, al4, vl);
-				// accumulator register ci <-> sample j: ci = ((j & 1) << 1) | (j >> 1)
-				#pragma unroll
-				for(int j = 0; j < 4; j++)
-				{
-					const int ci = mf_lane_ci(j);
-					cu[j] = kl_acc15(uhh[ci], umid[ci], ull[ci]);
-					cv[j] = kl_acc15(vhh[ci], vmid[ci], vll[ci]);
-					if(CSAT) { cu[j] = sat16i(cu[j]); cv[j] = sat16i(cv[j]); }
-				}
-			}
+			#pragma unroll
+			for(int j = 0; j < 4; j++) { cu[j] = (int) (short) (px[j] & 0xFFFFu); cv[j] = (int) px[j] >> 16; }
 			if(in_burst)
 			{
 				#pragma unroll
@@ -332,11 +254,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			}
 		}
 
-		const int rprev = r3 == 0 ? 2 : r3 - 1, rnext = r3 == 2 ? 0 : r3 + 1;
+		const int rprev = r4 == 0 ? 3 : r4 - 1, rnext = r4 == 3 ? 0 : r4 + 1;   // ring rows of lines q - 1, q + 1
 		if(VF)
 		{
-			// ---- composite line -> ring row q mod 3 (+ the neighbours' halos) ----------
-			unsigned char *rp = rows + (2 * r3) * RB + KL_LEAD + xb;
+			// ---- composite line -> ring row q mod 4 (+ the neighbours' halos) ----------
+			unsigned char *rp = rows + (2 * r4) * RB + KL_LEAD + xb;
 			#pragma unroll
 			for(int j = 0; j < 4; j++)
 			{
@@ -367,8 +289,8 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		if(tid < 4 + NA16) kl_cp_wait();
 		__syncthreads();                                                    // rows of line q, descriptors of q + 1 and of mrow
 
-		// ---- R1a: the next line's template and pixels start their way here -------------
-		if(q + 1 <= q1) KL_R1A(q + 1);
+		// ---- R1: the next line's values start their way here -------------------------
+		if(q + 1 <= q1) KL_R1(q + 1);
 		if(mrow < a) continue;
 
 		int oi[4], oq[4];
@@ -424,5 +346,5 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
 		}
 	}
-	#undef KL_R1A
+	#undef KL_R1
 }

@@ -297,6 +297,40 @@ static int build_templates(struct htv_tables_t *t)
 	return(0);
 }
 
+/* ---- picture rows (converted picture store) ------------------------------ *
+ * Which line of the frame shows each source picture row, with that line's picture geometry, so that a picture can be
+ * converted (RGB -> Y, U, V, chroma low-pass, the line template) row by row when it arrives, not line by line on every
+ * frame that shows it. The picture area [al, ar) of a line as the raster descriptors have it (k_line_desc_r): the whole
+ * active width, or half of it on the half lines. Lines with a picture area and no source row (a progressive picture
+ * on an interlaced raster, the 525-line raster's lines outside its 480 rows) draw black; each gets a row of its own
+ * behind the picture rows. -1: out of memory. */
+static int build_pic_rows(struct htv_tables_t *t)
+{
+	const htv_dparams_t *dp = &t->dp;
+	const int nl = dp->lines, ncap = dp->active_lines + nl;
+	int line, extra = 0;
+	t->line_row = malloc(sizeof(int32_t) * (nl + 1));
+	t->pic_rows = calloc((size_t) ncap * 4, sizeof(int32_t));
+	if(!t->line_row || !t->pic_rows) return(-1);
+	t->line_row[0] = -1;
+	for(line = 1; line <= nl; line++)
+	{
+		const int left = t->codes[line] & HTV_LC_LEFT_ACTIVE, right = t->codes[line] & HTV_LC_RIGHT_ACTIVE;
+		const int vy = htv_line_vy(dp, line);
+		int32_t *r;
+		t->line_row[line] = -1;
+		if(!left && !right) continue;
+		t->line_row[line] = vy >= 0 ? vy : dp->active_lines + extra++;
+		r = t->pic_rows + (size_t) t->line_row[line] * 4;
+		r[0] = line;
+		r[1] = left ? dp->active_left : dp->half_width;
+		r[2] = right ? dp->active_left + dp->active_width : dp->half_width;
+		r[3] = t->tmpl_keep_any[line - 1];
+	}
+	t->pic_nrows = dp->active_lines + extra;
+	return(0);
+}
+
 /* ---- the build --------------------------------------------------------- */
 
 static double dclamp(double v, double lo, double hi) { return(v < lo ? lo : (v > hi ? hi : v)); }
@@ -455,7 +489,7 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 	}
 
 	build_codes(t);
-	if(build_templates(t) != 0)
+	if(build_templates(t) != 0 || build_pic_rows(t) != 0)
 	{
 		fprintf(stderr, "hacktv_b200: out of memory for the line templates\n");
 		htv_tables_free(t);
@@ -877,7 +911,7 @@ void htv_tables_free(htv_tables_t *t)
 	if(!t) return;
 	free(t->rs_taps);
 	free(t->codes); free(t->pulse_values); free(t->clut); free(t->burst_win);
-	free(t->tmpl_out); free(t->tmpl_keep); free(t->tmpl_keep_any);
+	free(t->tmpl_out); free(t->tmpl_keep); free(t->tmpl_keep_any); free(t->pic_rows); free(t->line_row);
 	free(t->fm_ang); free(t->fm_rot8); free(t->fmv_ang); free(t->nicam_taps); free(t->nicam_tpad); free(t->nicam_lut); free(t->nicam_cc);
 	free(t->secam_fm_lut); free(t->secam_bell); free(t->offset_start); free(t->scratch);
 	free(t);
@@ -951,6 +985,8 @@ const int32_t *htv_tables_get(htv_tables_t *t, const char *name, int *count)
 		tmp[3] = dp->active_width; tmp[4] = dp->burst_left; tmp[5] = dp->burst_width;
 		return(view32(t, tmp, 6, count));
 	}
+	if(!strcmp(name, "pic_rows")) return(view32(t, t->pic_rows, 4 * t->pic_nrows, count));
+	if(!strcmp(name, "line_row")) return(view32(t, t->line_row, dp->lines + 1, count));
 	if(!strcmp(name, "codes"))
 	{
 		int i;
