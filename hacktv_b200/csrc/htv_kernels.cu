@@ -2442,7 +2442,32 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	if(p->line_threads < 64) p->line_threads = 64;
 	p->kl_threads = 32 * T;
 	if(p->line_threads > 384) { snprintf(err, errlen, "line width %d exceeds the kernels' 1536-sample limit", W); return(HTV_ERROR); }
+	// The lower limit: k_line's rows carry 32 samples of each neighbouring line (KL_LEAD halos), and the split modulators
+	// stage 32 samples of the line before (EXT), so a line shorter than that would take them from two lines back. FM
+	// video's k_fmv_base stages FOFF = 40 samples of the line before from the composite stream, which starts one line
+	// early: a shorter line would read in front of it.
+	if(W < 32) { snprintf(err, errlen, "line width %d is below the kernels' 32-sample limit", W); return(HTV_ERROR); }
+	if(dp.have_fmv && W < FOFF)
+	{
+		snprintf(err, errlen, "line width %d is below FM video's %d-sample limit", W, FOFF);
+		return(HTV_ERROR);
+	}
+	// kl_sound and the sound descriptors let at most one 32 kHz audio segment start in a 32-sample block
+	if((dp.have_fm || dp.have_am) && t->rate < 32u * 32000u)
+	{
+		snprintf(err, errlen, "FM / AM sound at %u Hz is below the kernels' 1.024 MHz limit (one audio sample per 32-sample block)", t->rate);
+		return(HTV_ERROR);
+	}
 	if(secam && t->rs_taps) { snprintf(err, errlen, "--pixelrate with SECAM is not on the accelerated path yet"); return(HTV_ERROR); }
+	// The video filter's taps ahead of centre reach the next line's first 25 samples. The SECAM chain of a call runs
+	// through the last line it emits, not the one after, so below about 5 Msps, where the burst window starts within
+	// those 25 samples, a call's last line would miss the next line's subcarrier.
+	if(secam && dp.vf_type && dp.burst_left < MF_NTAPS / 2)
+	{
+		snprintf(err, errlen, "SECAM with the video filter needs the burst window to start %d samples or more into the line "
+			"(it starts at %d)", MF_NTAPS / 2, dp.burst_left);
+		return(HTV_ERROR);
+	}
 	// The fused line kernel (htv_line.cuh) is the default wherever it applies: PAL / NTSC / mono rasters, AM or VSB
 	// modulation (or baseband), a chroma low-pass the tensor-core form holds (11 .. 17 taps), no resampler in front of
 	// this context. SECAM: its SRC form modulates what the raster and the chrominance chain wrote.

@@ -195,6 +195,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		// ---- descriptors of the next raster line and of the line modulated below -> shared memory -----
 		if(tid < 4) { if(!SRC && q + 1 <= q1) kl_cp16(reinterpret_cast<int4 *>(slr + ((q + 1) & 1)) + tid, reinterpret_cast<const int4 *>(lrp + q + 2) + tid); }
 		else if(tid < 4 + NA16) { if(mrow >= a) kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + (tid - 4), reinterpret_cast<const int4 *>(lap + mrow) + (tid - 4)); }
+		// a CTA narrower than 4 + NA16 threads (one warp: W <= 128) copies the rest of the descriptor in further passes;
+		// the forms with the width compiled in have 256 threads and need none
+		if(!WC && (int) blockDim.x < 4 + NA16 && mrow >= a)
+			for(int i = (int) blockDim.x - 4 + tid; i < NA16; i += blockDim.x)
+				kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + i, reinterpret_cast<const int4 *>(lap + mrow) + i);
 
 		// ---- R2: burst, subcarrier, VBI overlay of line q ---------------------------
 		const LineR2 &li = slr[q & 1];
@@ -286,7 +291,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 				}
 			}
 		}
-		if(tid < 4 + NA16) kl_cp_wait();
+		if(tid < 4 + NA16 || (!WC && (int) blockDim.x < 4 + NA16)) kl_cp_wait();
 		__syncthreads();                                                    // rows of line q, descriptors of q + 1 and of mrow
 
 		// ---- R1: the next line's values start their way here -------------------------

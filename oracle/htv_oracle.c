@@ -13,6 +13,7 @@
 #define I16MAX 32767
 #define I16MIN (-32768)
 #define I32MAX 2147483647
+#define ORC_RING 8      /* composite lines held: t - 1 .. t + 3 while line t is emitted (SECAM rasters one further) */
 
 typedef struct { int16_t i, q; } c16_t;
 typedef struct { int32_t i, q; } c32_t;
@@ -368,6 +369,15 @@ struct orc_t {
 	int16_t *secam_notch;       /* 51 taps */
 	int16_t secam_dmin[2], secam_dmax[2];
 	c16_t *secam_bell;          /* 65536 */
+	/* The reference's line buffers (video.c:4642-4672) are a ring of `olines`, each with the zero heap's padding past
+	 * its W samples. Where the burst window ends past the line (82 + 944 > 1024 at 16 Msps), the subcarrier loop adds
+	 * into that padding (video.c:3228), and it is never cleared: what a ring buffer's past SECAM lines added there is
+	 * what the luma notch of its next SECAM line reads through its taps ahead of centre, wherever the picture ends
+	 * within 25 samples of the line's end (below about 15 Msps; it changes values below about 10). I of samples W, W + 1,
+	 * ... per ring buffer. Restated only on request (orc_set_ref_heap) and without a resampler, whose wider output
+	 * lines share the ring; otherwise the notch reads zeros past the line, as the CUDA path does. */
+	int ref_heap, olines;
+	int16_t secam_pad[32][8];
 
 	/* video filter: ref video.c:3653-3764 */
 	int vf_type;                /* 0 none, 1 real, 3 real->complex */
@@ -402,7 +412,7 @@ struct orc_t {
 	int64_t next_raster;        /* next line index to raster */
 	int64_t next_secam;         /* next line index for the SECAM pass */
 	int64_t next_emit;          /* next line index to emit */
-	int16_t *ring[4];           /* composite I, W + pad each */
+	int16_t *ring[ORC_RING];    /* composite I, W + pad each */
 
 	/* --pixelrate: the raster side (everything above) runs at `rate` / `width`, the stages from the
 	 * resampler on at `srate` / `swidth` (ref video.c:3839-3853, 4361-4368). Equal without a resampler. */
@@ -949,7 +959,7 @@ static const uint32_t *frame_for(const orc_t *o, int frame /* 1-based */)
 /* Raster: ref video.c:2864-3066, vbidata.c:186-239                         */
 /* ------------------------------------------------------------------------ */
 
-static inline int16_t *ring_line(orc_t *o, int64_t L) { return(o->ring[((L % 4) + 4) % 4]); }
+static inline int16_t *ring_line(orc_t *o, int64_t L) { return(o->ring[((L % ORC_RING) + ORC_RING) % ORC_RING]); }
 
 static void blank_line(orc_t *o, int16_t *l)
 {
@@ -1087,12 +1097,37 @@ static void vbi_line(orc_t *o, int64_t L)
 /* SECAM chroma: ref video.c:3068-3233                                      */
 /* ------------------------------------------------------------------------ */
 
-static void secam_line(orc_t *o, int16_t *l, int frame, int line)
+/* The reference's line-buffer count: _add_lineprocess (video.c:3543-3579) over the stages vid_init adds
+ * (video.c:4206-4638) for what the oracle restates, as (lines, threaded) in their order. A stage that is not threaded
+ * shares its first line with the unthreaded stage before it. */
+static int ref_olines(const orc_t *o)
+{
+	int st[12][2], n = 0, i, total = 0;
+	st[n][0] = 3; st[n++][1] = 0;                                    /* raster */
+	st[n][0] = 1; st[n++][1] = 1;                                    /* secam */
+	if(o->nvbi) { st[n][0] = 1; st[n++][1] = 0; }                    /* wss */
+	if(o->rs_on) { st[n][0] = 2; st[n++][1] = 1; }                   /* vresampler */
+	if(o->vf_type)                                                   /* vfilter: 1 + its delay (video.c:3759) */
+		{ st[n][0] = 1 + (o->vf_ntaps / 2 + o->swidth - 1) / o->swidth; st[n++][1] = 1; }
+	st[n][0] = 1; st[n++][1] = 1;                                    /* audio */
+	if(o->have_fmv) { st[n][0] = 1; st[n++][1] = 1; }                /* fmmod */
+	if(o->p.swap_iq) { st[n][0] = 1; st[n++][1] = 0; }               /* swap_iq */
+	if(o->p.offset != 0) { st[n][0] = 1; st[n++][1] = 1; }           /* offset */
+	if(o->pt) { st[n][0] = 1; st[n++][1] = 0; }                      /* passthru */
+	st[n][0] = 1; st[n++][1] = 0;                                    /* output */
+	for(i = 0; i < n; i++) total += st[i][0] - (i == 0 || st[i][1] || st[i - 1][1] ? 0 : 1);
+	return(total);
+}
+
+/* SECAM on raster line L of the stream (the two fill buffers in front of it are -2 and -1): L is what places it in the
+ * reference's ring of line buffers, whose padding it reads and adds to */
+static void secam_line(orc_t *o, int16_t *l, int64_t L, int frame, int line)
 {
 	const int W = o->width;
 	const char *seq = line_code(o->p.type, line);
 	int vy = source_row(o, line);
 	int16_t *cb = o->chroma;
+	int16_t *pad = o->secam_pad[((L % o->olines) + o->olines) % o->olines];
 	int sl = 0, sr = 0, x;
 	int dr = ((frame * o->p.lines) + line) & 1;
 
@@ -1123,10 +1158,11 @@ static void secam_line(orc_t *o, int16_t *l, int frame, int line)
 	if(sr > sl)
 	{
 		int16_t dmin, dmax;
-		int16_t dummy = 0;
 
-		/* luma notch over the active region, in place, step 1 here (I only) */
+		/* luma notch over the active region, in place, step 1 here (I only); past the line it reads the padding */
+		if(o->ref_heap) for(x = 0; x < 8; x++) l[W + x] = pad[x];
 		fir_block(o->secam_notch, 51, l + o->active_left, l + o->active_left, o->active_width, 1);
+		for(x = 0; x < 8; x++) l[W + x] = 0;
 		fir_block(o->secam_lpf, 15, cb, cb, W, 1);
 
 		/* ref fir.c:721-735 - double IIR, state carried across processed lines */
@@ -1155,11 +1191,10 @@ static void secam_line(orc_t *o, int16_t *l, int frame, int line)
 			g = &o->secam_bell[(uint16_t) cb[x]];
 			fm_cgain(&o->fm_secam, &cb[x], cb[x], g);
 			/* x can reach W, W+1 (burst window 82+944 > 1024): the reference
-			 * then writes past the line buffer (video.c:3228); discard */
+			 * then writes into the line buffer's padding (video.c:3228) */
 			if(x < W) l[x] += (cb[x] * o->burst_win[x - o->burst_left]) >> 15;
-			else dummy += (cb[x] * o->burst_win[x - o->burst_left]) >> 15;
+			else if(x < W + 8) pad[x - W] += (cb[x] * o->burst_win[x - o->burst_left]) >> 15;
 		}
-		(void) dummy;
 	}
 }
 
@@ -1551,7 +1586,16 @@ orc_t *orc_open2(const orc_params_t *params, unsigned int sample_rate, unsigned 
 		o->off_delta.q = lround(sin(d) * I32MAX);
 	}
 
-	for(i = 0; i < 4; i++)
+	/* the filter stage's delay is (ntaps / 2 + W - 1) / W lines (ref video.c:3759) and the render here assumes one: two
+	 * lines below W = ntaps / 2 (25 at 51 taps). At W = ntaps / 2 the delay is one line, but the stream still differs from
+	 * the reference's (51 taps, W = 25: not restated), so the refusal starts there. */
+	if(o->vf_type && o->swidth <= o->vf_ntaps / 2)
+	{
+		orc_close(o);
+		return(NULL);
+	}
+
+	for(i = 0; i < ORC_RING; i++)
 	{
 		o->ring[i] = calloc((o->swidth > o->width ? o->swidth : o->width) + 64, sizeof(int16_t));
 		blank_line(o, o->ring[i]);
@@ -1565,7 +1609,8 @@ void orc_close(orc_t *o)
 	int i;
 	if(!o) return;
 	for(i = 0; i < 5; i++) free(o->syncs[i].value);
-	for(i = 0; i < 4; i++) { free(o->ring[i]); free(o->rring[i]); }
+	for(i = 0; i < ORC_RING; i++) free(o->ring[i]);
+	for(i = 0; i < 4; i++) free(o->rring[i]);
 	free(o->rs_taps);
 	free(o->clut); free(o->chroma); free(o->chroma_taps); free(o->burst_win);
 	free(o->fm_secam.lut); free(o->secam_lpf); free(o->secam_notch); free(o->secam_bell);
@@ -1581,6 +1626,7 @@ void orc_close(orc_t *o)
 	free(o);
 }
 
+void orc_set_ref_heap(orc_t *o, int on) { o->ref_heap = on && !o->rs_on; }
 void orc_set_frames(orc_t *o, const uint32_t *rgb, int nframes) { o->frames = rgb; o->nframes = nframes; }
 void orc_add_vbi_line(orc_t *o, int line, int replace_from, int replace_to, int replace_value, const int16_t *add)
 {
@@ -1647,10 +1693,11 @@ size_t orc_render(orc_t *o, int nlines, int16_t *out)
 		if(o->p.colour_mode == ORC_COLOUR_SECAM)
 		{
 			int16_t *fill = calloc((o->swidth > o->width ? o->swidth : o->width) + 64, sizeof(int16_t));
+			o->olines = ref_olines(o);
 			for(k = 0; k < 2; k++)
 			{
 				blank_line(o, fill);
-				secam_line(o, fill, 1, 0);
+				secam_line(o, fill, k - 2, 1, 0);
 			}
 			free(fill);
 		}
@@ -1719,7 +1766,7 @@ size_t orc_render(orc_t *o, int nlines, int16_t *out)
 					while(o->next_secam <= L)
 					{
 						int64_t M = o->next_secam++;
-						secam_line(o, ring_line(o, M), M / o->p.lines + 1, M % o->p.lines + 1);
+						secam_line(o, ring_line(o, M), M, M / o->p.lines + 1, M % o->p.lines + 1);
 					}
 				}
 				if(o->nvbi) vbi_line(o, L);
@@ -1735,13 +1782,16 @@ size_t orc_render(orc_t *o, int nlines, int16_t *out)
 		/* raster through t+1 (sync back-spill, filter look-ahead) */
 		while(o->next_raster <= t + 1) raster_line(o, o->next_raster++);
 
-		/* SECAM sees a line only after the following line's raster */
+		/* SECAM sees a line only after the following line's raster. It runs ahead of the video filter in the
+		 * reference's pipeline, so the filter's taps ahead of centre find line t + 1 with its subcarrier: below about
+		 * 5 Msps the burst window starts within them (20 < 25 samples at 4 Msps). */
 		if(o->p.colour_mode == ORC_COLOUR_SECAM)
 		{
-			while(o->next_secam <= t)
+			while(o->next_raster <= t + 2) raster_line(o, o->next_raster++);
+			while(o->next_secam <= t + 1)
 			{
 				int64_t L = o->next_secam++;
-				secam_line(o, ring_line(o, L), L / o->p.lines + 1, L % o->p.lines + 1);
+				secam_line(o, ring_line(o, L), L, L / o->p.lines + 1, L % o->p.lines + 1);
 			}
 		}
 

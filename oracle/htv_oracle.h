@@ -126,6 +126,9 @@ extern void orc_close(orc_t *o);
 /* AV source (reference av.h:64-116 callbacks, flattened): frames are RGB32
  * active_width x active_lines, used cyclically one per video frame; audio is
  * 32 kHz stereo int16, used cyclically. Pointers are borrowed. */
+/* SECAM: let the luma notch read what the reference's subcarrier loop left past the end of earlier lines in its line
+ * buffers' zero-heap padding (ref video.c:3206, 3228), as the reference does, instead of zeros. Not with --pixelrate. */
+extern void orc_set_ref_heap(orc_t *o, int on);
 extern void orc_set_frames(orc_t *o, const uint32_t *rgb, int nframes);
 extern void orc_set_audio(orc_t *o, const int16_t *pcm, size_t npairs);
 /* External int16 complex stream added to the output (ref --passthru, video.c:3517-3541);

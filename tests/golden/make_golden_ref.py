@@ -73,6 +73,13 @@ def main():
         run(mode, rate, nlines, vfilter=filt, extra=extra, source=f"programme{seed}", frames=frames, audio=audio,
             audio_block=block)
 
+    for mode, rate, nlines in T.LOW_RATE_SOURCES:
+        o = orc.Oracle(H.mode_config(mode, vfilter=True), rate)
+        frames, audio = T.random_source(13, o.active_lines, o.active_width)
+        run(mode, rate, nlines, vfilter=True, source="random13", frames=frames, audio=audio)
+        frames, audio = T.programme_source(17, o.active_lines, o.active_width)
+        run(mode, rate, nlines, vfilter=True, source="programme17", frames=frames, audio=audio)
+
     raw = orc.run_ref("i", 16000000, 700, vfilter=True, rawheap=True)
     put(T.ref_key("i", 16000000, 700, vfilter=True, rawheap=True), raw,
         masked_32_sha256=hashlib.sha256(np.ascontiguousarray(raw.reshape(700, 1024, 2)[:, 32:-32]).tobytes()).hexdigest())

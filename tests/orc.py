@@ -27,6 +27,7 @@ def lib():
         L.orc_open.restype = vp; L.orc_open.argtypes = [vp, C.c_uint]
         L.orc_open2.restype = vp; L.orc_open2.argtypes = [vp, C.c_uint, C.c_uint]
         L.orc_close.restype = None; L.orc_close.argtypes = [vp]
+        L.orc_set_ref_heap.restype = None; L.orc_set_ref_heap.argtypes = [vp, C.c_int]
         L.orc_set_frames.restype = None; L.orc_set_frames.argtypes = [vp, vp, C.c_int]
         L.orc_set_audio.restype = None; L.orc_set_audio.argtypes = [vp, vp, C.c_size_t]
         L.orc_set_passthru.restype = None; L.orc_set_passthru.argtypes = [vp, vp, C.c_size_t]
@@ -47,13 +48,16 @@ class Oracle:
     """orc_t. `conf` is a hacktv_b200.Config: htv_config_t and orc_params_t share one layout
     (checked against orc_params_size())."""
 
-    def __init__(self, conf, sample_rate, pixel_rate=0):
+    def __init__(self, conf, sample_rate, pixel_rate=0, ref_heap=False):
+        """ref_heap: SECAM's luma notch reads what the reference left in its line buffers' padding, not zeros
+        (orc_set_ref_heap); the reference's stream, where the CUDA path's differs near the picture's right edge."""
         L = lib()
         assert C.sizeof(conf) == L.orc_params_size(), "orc_params_t / htv_config_t layouts differ"
         self._L = L
         self._o = L.orc_open2(C.byref(conf), sample_rate, pixel_rate)
         if not self._o:
             raise RuntimeError("orc_open failed")
+        L.orc_set_ref_heap(self._o, int(ref_heap))
         self.width = L.orc_width(self._o)
         self.raster_width = L.orc_raster_width(self._o)    # differs from width with a --pixelrate resampler
         self.active_width = L.orc_active_width(self._o)

@@ -81,8 +81,25 @@ def _mode_matrix_cases():
     return out
 
 
+def _low_rate_cases():
+    """Every row of the device's low-rate matrix (test_gpu_zz_low_rates.py), with the mode's sound and the lines it
+    renders."""
+    from test_gpu_zz_low_rates import MATRIX
+    out = []
+    for mode, rate, kw, _, _ in MATRIX:
+        extra = tuple(f"--{k}" for k in ("nocolour", "nonicam", "noaudio") if kw.get(k))
+        case = (mode, rate, 290 if mode in ("m", "ntsc") else 340, bool(kw.get("vfilter")), extra)
+        if case not in CASES and case not in out:
+            out.append(case)
+    return out
+
+
 CASES += _line_width_cases()
 CASES += _mode_matrix_cases()
+CASES += _low_rate_cases()
+# SECAM with the video filter below 5 Msps: the filter's taps ahead reach the next line's burst window (the device
+# refuses these; the oracle restates them)
+CASES += [("l", 4000000, 340, True, ()), ("l", 2000000, 340, True, ())]
 
 
 def ref_key(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", rawheap=False):
@@ -153,13 +170,26 @@ def _conf(H, mode, filt, extra):
     return H.mode_config(mode, **kw)
 
 
+# SECAM cases whose reference stream depends on the heap padding past the line that the reference's luma notch reads
+# (DESIGN.md section 2): there the oracle's default, which reads zeros as the CUDA path does, differs from it
+HEAP_CASES = {("secam", 6000000), ("secam", 8000000), ("secam", 9000000), ("secam", 10000000), ("l", 8000000)}
+
+
 @pytest.mark.parametrize("mode,rate,nlines,filt,extra", CASES)
 def test_oracle_equals_reference(built, mode, rate, nlines, filt, extra):
-    o = orc.Oracle(_conf(built, mode, filt, extra), rate)
-    o.open_test_source()
-    got = o.render(nlines)
-    o.close()
-    assert_reference(got, ref_key(mode, rate, nlines, vfilter=filt, extra=extra))
+    """The oracle's default is the reference's stream everywhere but HEAP_CASES, where it differs; with ref_heap (SECAM
+    only) it is the reference's stream in every case."""
+    conf = _conf(built, mode, filt, extra)
+    key = ref_key(mode, rate, nlines, vfilter=filt, extra=extra)
+    for ref_heap in (False, True) if conf.colour_mode == 3 else (False,):
+        o = orc.Oracle(conf, rate, ref_heap=ref_heap)
+        o.open_test_source()
+        got = o.render(nlines)
+        o.close()
+        if ref_heap or (mode, rate) not in HEAP_CASES:
+            assert_reference(got, key)
+        else:
+            assert digest(got) != golden_ref()[key]["sha256"], "the default no longer differs: is the case in HEAP_CASES?"
 
 
 PASSTHRU_CASES = [
@@ -225,6 +255,53 @@ def test_oracle_equals_reference_on_random_input(built):
     got = o.render(1400)
     o.close()
     assert_reference(got, ref_key("i", 16000000, 1400, vfilter=True, source="random7"))
+
+
+# low rates the random and the programme source are pinned at: 3 chroma taps on k_line, and 1 Msps (64 samples a
+# line, a 32 kHz audio sample every 31.25 samples: the device refuses sound there, the oracle restates it)
+LOW_RATE_SOURCES = [("i", 2000000, 700), ("i", 1000000, 700)]
+
+
+@pytest.mark.parametrize("mode,rate,nlines", LOW_RATE_SOURCES)
+def test_oracle_equals_reference_on_random_input_at_low_rates(built, mode, rate, nlines):
+    o = orc.Oracle(built.mode_config(mode, vfilter=True), rate)
+    frames, audio = random_source(13, o.active_lines, o.active_width)
+    o.set_source(frames, audio)
+    got = o.render(nlines)
+    o.close()
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=True, source="random13"))
+
+
+@pytest.mark.parametrize("mode,rate,nlines", LOW_RATE_SOURCES)
+def test_oracle_equals_reference_on_programme_audio_at_low_rates(built, mode, rate, nlines):
+    o = orc.Oracle(built.mode_config(mode, vfilter=True), rate)
+    o.set_source(*programme_source(17, o.active_lines, o.active_width))
+    got = o.render(nlines)
+    o.close()
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=True, source="programme17"))
+
+
+def test_secam_notch_reads_the_reference_heap_padding(built):
+    """SECAM at 6 Msps: the reference's luma notch reads the padding past its line buffer, which holds what the
+    subcarrier loop of earlier lines added past the burst window's end there. ref_heap restates that (the reference's
+    stream); without it the notch reads zeros, as the CUDA path does, and the two streams differ only in the last 25
+    samples of the picture."""
+    conf = built.mode_config("secam")
+    outs = []
+    for ref_heap in (True, False):
+        o = orc.Oracle(conf, 6000000, ref_heap=ref_heap)
+        o.open_test_source()
+        outs.append(o.render(340))
+        aw, W = o.active_width, o.width
+        o.close()
+    assert_reference(outs[0], ref_key("secam", 6000000, 340))
+    d = (outs[0] != outs[1]).reshape(340, W)
+    assert d.any()
+    x = np.flatnonzero(d.any(axis=0))
+    t = built.Tables(conf, 6000000)
+    end = int(t.get("geometry")[2]) + aw                      # the picture's end: 62 + 312
+    t.close()
+    assert x.min() >= end - 25 and x.max() < end, x
 
 
 def programme_cases():

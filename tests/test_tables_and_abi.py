@@ -337,3 +337,80 @@ def test_c_selection_of_the_scalar_video_filter(built):
     assert _plan_name(built, "i", 16000000, F, HTV_FIR="scalar") == "k_raster + k_mod_tma<256,4>"
     assert _plan_name(built, "l", 16000000, F, HTV_FIR="scalar") == \
         "k_raster_secam + k_line<VF=1,HQ=1,FULL=1,CSAT=0,MAXT=256,SRC=1,SND=-1,WC=0>"
+
+
+def test_c_selection_runs_what_the_low_rate_matrix_asserts(built):
+    """The GPU low-rate matrix (test_gpu_zz_low_rates.py) without a GPU: every row's W is what the tables give and the C
+    selection names the kernels the row asserts; together the rows reach chroma low-pass lengths 1, 3, 5 and 7, a CSAT
+    rate, k_line at W <= 128 (a single-warp CTA) and at the 32-sample limit, every split modulator, and SECAM at
+    W <= 128."""
+    from test_gpu_zz_low_rates import MATRIX
+    taps, csat, narrow, mods, secam = set(), False, set(), set(), set()
+    for mode, rate, kw, W, kernel in MATRIX:
+        t = built.Tables(built.mode_config(mode, **kw), rate)
+        w, ct = int(t.get("geometry")[0]), t.get("chroma_taps")
+        t.close()
+        what = f"{mode} {rate} {kw}"
+        assert w == W, (what, w)
+        assert _plan_name(built, mode, rate, kw) == kernel, what
+        if ct is not None and kernel.startswith(("k_line", "k_raster + ")):
+            taps.add(len(ct))
+            csat |= "CSAT=1" in kernel and int(np.abs(ct).sum()) > 32768
+        if kernel.startswith("k_line") and W <= 128:
+            narrow.add(W)
+        mods |= {m for m in ("k_mod_tma", "k_mod_mma", "k_mod<") if m in kernel}
+        if kernel.startswith("k_sec_raster"):
+            secam.add(W)
+    assert taps >= {1, 3, 5, 7} and csat, (taps, csat)
+    assert {32, 96, 128} <= narrow, narrow
+    assert mods == {"k_mod_tma", "k_mod_mma", "k_mod<"}, mods
+    assert min(secam) <= 128, secam
+
+
+@pytest.mark.parametrize("mode,rate,kw,W,kernel", [
+    ("i", 500000, dict(vfilter=True, nocolour=True, noaudio=True), 32, "k_line<"),
+    ("pal", 500000, {}, 32, "k_raster + k_mod_tma<"),
+    ("pal", 500000, dict(vfilter=True), 32, "k_raster + k_mod_mma<"),
+    ("ntsc", 500000, {}, 32, "k_raster + k_mod_tma<"),
+    ("secam", 500000, {}, 32, "k_sec_raster<"),
+    ("pal-fm", 625000, dict(vfilter=True, noaudio=True), 40, "k_fmv_base<"),
+    ("i", 1024000, dict(vfilter=True), 66, "k_mod_mma<"),
+    ("l", 5000000, dict(vfilter=True), 320, "k_sec_raster<"),
+])
+def test_lower_width_limit(built, mode, rate, kw, W, kernel):
+    """The smallest line each path holds is selected, and the one just below it refused with the limit's message:
+    32 samples for k_line, the split modulators and SECAM; 40 for FM video, whose k_fmv_base stages FOFF = 40 samples of
+    the line before; FM / AM sound 1.024 MHz; SECAM with the video filter 5 Msps, where the burst window starts 25
+    samples into the line."""
+    import ctypes as C
+    H = built
+    t = H.Tables(H.mode_config(mode, **kw), rate)
+    assert int(t.get("geometry")[0]) == W
+    t.close()
+    assert kernel in _plan_name(H, mode, rate, kw)
+    below = {1024000: 1023000, 5000000: 4750000}.get(rate, rate - 15625)
+    t = H.Tables(H.mode_config(mode, **kw), below)
+    buf = C.create_string_buffer(256)
+    assert H.lib().htv_dev_plan_name(t._t, H.SAMPLE_TYPES["int16"], buf, len(buf)) != H.HTV_OK
+    t.close()
+    msg = buf.value.decode()
+    if rate == 1024000:
+        assert "FM / AM sound at 1023000 Hz is below the kernels' 1.024 MHz limit" in msg, msg
+    elif mode == "l":
+        assert "SECAM with the video filter needs the burst window to start 25 samples or more into the line " \
+            "(it starts at 24)" in msg, msg
+    elif mode == "pal-fm":
+        assert f"line width {W - 1} is below FM video's {W}-sample limit" in msg, msg
+    else:
+        assert f"line width {W - 1} is below the kernels' 32-sample limit" in msg, msg
+
+
+def test_oracle_refuses_a_line_shorter_than_the_filter_delay(built):
+    """Below 25 samples the reference delays the filtered stream by two lines ((25 + W - 1) / W, ref video.c:3759). At
+    W = 25 the delay is one line, but the oracle's stream is not the reference's there (51 taps reach exactly one whole
+    line ahead), so the oracle restates W >= 26 and refuses W <= 25."""
+    conf = built.mode_config("i", vfilter=True, nocolour=True, noaudio=True)
+    orc.Oracle(conf, 406250).close()                                 # W = 26
+    for rate in (390625, 375000):                                    # W = 25, 24
+        with pytest.raises(RuntimeError):
+            orc.Oracle(conf, rate)
