@@ -117,12 +117,15 @@ struct htv_tables_t {
 	int16_t *pulse_values;  int npulse_values;
 	int16_t *tmpl_out, *tmpl_keep;                 /* [tmpl_rows][W] line templates: blank + sync pulses (htv_tables.c) */
 	uint8_t *tmpl_keep_any; int tmpl_rows;         /* lines + 2 */
-	/* rows of the converted picture store (htv_tables.c build_pic_rows): pic_rows[row] = line (1-based, 0: no line draws
+	/* rows of the converted picture store, which the fused line kernel keeps for encoders whose colour subcarrier does not
+	 * repeat within 4 frames (comp_phases = 0; htv_tables.c build_pic_rows): pic_rows[row] = line (1-based, 0: no line draws
 	 * the row), al, ar, keep of the line that shows it; rows 0 .. active_lines - 1 are the picture rows, the rest the
 	 * lines with a picture area and no source row (always black). line_row[line] = the row line `line` shows, -1: the
 	 * line has no picture area. */
 	int32_t *pic_rows;      int pic_nrows;
 	int32_t *line_row;
+	int comp_phases;        /* frames after which a line's colour subcarrier, V-switch and burst repeat (1, 2 or 4; 0: more:
+	                         * no composite store, k_line's PS forms) */
 	double glut[256];
 	htv_c16_t *clut;        size_t clut_len;      /* clut_width + W */
 	int16_t *burst_win;     int burst_width;

@@ -82,8 +82,15 @@ struct DevTables {
 	const int32_t *frame_map;         // slot of frame (first_frame + i)
 	int64_t frame_map_first;          // 0-based frame index of frame_map[0]
 	int32_t frame_map_len;
-	// converted picture store of the fused line kernel (k_picture): [slot][row][W], slot max_slots = black, row as
-	// htv_tables.c build_pic_rows; NULL on every other path
+	// composite store of the fused line kernel (k_compose): every line of the frame as the finished composite row before
+	// the VBI overlay and the video filter, [slot][phase][line - 1][W], slot max_slots = black, phase = frame mod
+	// comp_phases, then the two stream-start rows (comp_start: L < 0, comp_start + 1: L = 0); NULL on every other path
+	int16_t *comp;
+	int16_t *comp_q;                  // S-Video: the chroma term of each row (Q), same layout; NULL otherwise
+	int32_t comp_phases, comp_black;  // colour-frame phases; the black slot
+	int64_t comp_start;               // row of the first stream-start row
+	// converted picture store of the k_line encoders whose subcarrier does not repeat within 4 frames (k_picture; k_line's
+	// PS forms): [slot][row][W], slot max_slots = black, row as htv_tables.c build_pic_rows; NULL on every other path
 	const int4 *pic_rows;             // [pic_nrows] line (1-based, 0 none), al, ar, keep of the line that shows the row
 	const int32_t *line_row;          // [lines + 1] the row line l shows, -1: no picture area
 	int32_t pic_nrows, pic_black;     // rows per slot; the black slot
@@ -212,8 +219,11 @@ struct htv_dev_t {
 	cudaEvent_t ev_nic;
 	cudaStream_t up;                  // picture / PCM uploads: ahead of the previous chunk's kernels
 	cudaEvent_t ev_up, ev_chunk[2];
-	cudaStream_t pic;                 // the converted picture store (k_picture), behind each picture's copy but off the
-	cudaEvent_t ev_copied, ev_pic;    // upload stream, so that the next copies do not queue behind the conversions
+	cudaStream_t pic;                 // the conversions (k_compose, k_picture), each behind its picture's copy but off the
+	cudaEvent_t ev_pic;               // upload stream, so that the next copies do not queue behind the conversions
+	cudaEvent_t *ev_slot;             // [max_slots] the copy of each slot's last picture is done
+	uint8_t *comp_valid;              // [max_slots] the phases of each slot's composite rows that hold its picture (bit p)
+	int pic_pending;                  // conversions were launched that the caller's stream has not waited for yet
 	unsigned chunk_i;
 	cudaEvent_t ev_in, ev_audio;
 	cudaEvent_t ev_kl[2];             // the fused line kernel has read descriptor buffer 0 / 1
@@ -648,8 +658,7 @@ struct __align__(16) LineR2 {
 	unsigned int clut_off;
 	int ov_to, ov_value, ov_add;      // ov_add: row of dt.ov_add, -1 none; ov_from >= ov_to: no replace
 	long long row_off;                // pixel offset of the source row in the frame store, -1 = black
-	long long pic;                    // k_line: offset of the line's row in the converted picture store (dt.pic_val,
-	                                  // dt.pic_cuv), -1: no picture area, the template row is the line
+	long long pic;                    // k_line: offset of the line's row in the composite store (dt.comp, dt.comp_q)
 };
 static_assert(sizeof(LineR2) == 64, "LineR2 is read as four int4");
 
@@ -778,13 +787,23 @@ __global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const De
 	o.ov_any = line_overlay(dt, L, m);
 	o.ov_from = m.x; o.ov_to = m.y; o.ov_value = m.z; o.ov_add = m.w;
 	o.row_off = row_off;
-	// the converted row: of the frame's picture, of the black slot where the frame has none or the line no source row
+	// the composite row: of the frame's picture at its colour-frame phase, of the black slot where the frame has none
 	o.pic = -1;
 	if(dt.pic_val && al < ar)
 	{
 		const int row = dt.line_row[line];
 		const int slot = row < dp.active_lines ? frame_slot(dt, frame - 1) : -1;
 		o.pic = ((long long) (slot >= 0 ? slot : dt.pic_black) * dt.pic_nrows + row) * dp.W;
+	}
+	if(dt.comp)
+	{
+		long long row = dt.comp_start + (L < 0 ? 0 : 1);
+		if(L > 0)
+		{
+			const int slot = frame_slot(dt, frame - 1);
+			row = ((long long) (slot >= 0 ? slot : dt.comp_black) * dt.comp_phases + (frame - 1) % dt.comp_phases) * dp.lines + line - 1;
+		}
+		o.pic = row * dp.W;
 	}
 	reinterpret_cast<LineR2 *>(out)[i] = o;
 }
@@ -1191,7 +1210,7 @@ __device__ __forceinline__ void store_line4(const int (&val)[SPT], int x0, int W
 
 // A thread's line values x0 .. x0 + 3 before the subcarrier (ref video.c:2864-2992): row `tmpl` of the line templates
 // outside the picture area [al, ar), the picture's Y plus the template's keep part inside it; U, V inside it, 0 outside.
-// rgb: the source row (pixel x at rgb[x - active_left]), NULL: black. k_raster and k_picture raster through here.
+// rgb: the source row (pixel x at rgb[x - active_left]), NULL: black. k_raster and k_compose raster through here.
 __device__ __forceinline__ void raster_pic4(const htv_dparams_t &dp, const DevTables &dt, int tmpl, int al, int ar, bool keep,
 	const uint32_t *rgb, int x0, int (&val)[SPT], int (&uu)[SPT], int (&vv)[SPT])
 {
@@ -1319,9 +1338,10 @@ k_raster(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Lin
 }
 
 // ---------------------------------------------------------------------------
-// Converted picture store of the fused line kernel: the part of a line that depends on the picture and on the line's
-// place in the frame only - the line template, Y, and U / V through the chroma low-pass - converted once per picture
-// when it arrives (htv_dev_upload_frame[s]), not on every line that shows it. One CTA per row `blockIdx.x` of picture
+// Converted picture store of the fused line kernel's PS forms (encoders whose subcarrier does not repeat within 4
+// frames): the part of a line that depends on the picture and on the line's place in the frame only - the line
+// template, Y, and U / V through the chroma low-pass - converted once per picture when it arrives
+// (htv_dev_upload_frame[s]), not on every line that shows it. One CTA per row `blockIdx.x` of picture
 // slot `slot0 + blockIdx.y` (slot max_slots, the black slot: from zero RGB), 4 samples per thread, as k_raster's first
 // half; the line of the row and its geometry come from the host (htv_tables.c build_pic_rows). What k_line takes from
 // here is what k_raster computes up to the burst: dt.pic_val = val[], dt.pic_cuv = (cu, cv) over the whole line.
@@ -1367,6 +1387,100 @@ k_picture(const __grid_constant__ htv_dparams_t dp, const DevTables dt, int slot
 	for(int k = 0; k < SPT; k++) w[k] = ((unsigned) cu[k] & 0xFFFFu) | ((unsigned) cv[k] << 16);
 	if((W & 3) == 0) *reinterpret_cast<uint4 *>(dt.pic_cuv + at) = make_uint4(w[0], w[1], w[2], w[3]);
 	else for(int k = 0; k < SPT; k++) if(x0 + k < W) dt.pic_cuv[at + k] = w[k];
+}
+
+// ---------------------------------------------------------------------------
+// Composite store of the fused line kernel: everything of a line that depends on the picture, the line's place in the
+// frame and the colour-frame phase only - the line template, Y, U / V through the chroma low-pass, burst and subcarrier
+// (ref video.c:2864-3040) - converted once per (picture, phase) the frames that show the picture need
+// (htv_dev_set_frame_map), not on every line of every frame. The subcarrier offset (L W mod clut_width), V-switch and
+// burst code of line `line` of frame f0 (0-based) depend on f0 mod comp_phases only (htv_tables.c).
+// One CTA per line `blockIdx.x + 1` of slot `slot` at phase `phase` (slot max_slots, the black slot: from zero RGB), 4
+// samples per thread, as k_raster. start: the two stream-start rows instead (block 0: the lines before the stream, block
+// 1: stream line 0, which has templates of their own; neither has a picture area, htv_dev_create checks).
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(384)
+k_compose(const __grid_constant__ htv_dparams_t dp, const DevTables dt, int slot, int phase, int start)
+{
+	extern __shared__ __align__(16) unsigned char smem_raw[];
+	const int W = dp.W, W4 = (W + 3) & ~3;
+	int *su = reinterpret_cast<int *>(smem_raw);                    // index = x + UOFF
+	int *sv = su + W4 + 2 * UOFF;
+	const int tid = threadIdx.x;
+	const int line = start ? 1 : blockIdx.x + 1, frame = phase + 1;
+	const int code = start && blockIdx.x == 0 ? 0 : dt.codes[line];
+	const int left = code & HTV_LC_LEFT_ACTIVE, right = code & HTV_LC_RIGHT_ACTIVE;
+	const int al = left ? dp.active_left : (right ? dp.half_width : -1);
+	const int ar = right ? dp.active_left + dp.active_width : (left ? dp.half_width : -1);
+	const int tmpl = start ? dp.lines + 1 - blockIdx.x : line - 1;
+	const int vy = htv_line_vy(&dp, line);
+	const uint32_t *rgb = slot == dt.comp_black || vy < 0 ? NULL : dt.frames + ((size_t) slot * dp.active_lines + vy) * dp.active_width;
+	// V-switch and subcarrier offset as k_line_desc_r has them for a line of a frame f0 with f0 mod comp_phases = phase
+	int pal = 0;
+	unsigned clut_off = 0;
+	if(code && (dp.colour_mode == HTV_PAL || dp.colour_mode == HTV_NTSC))
+	{
+		const int b = (code & HTV_LC_BURST_MASK) >> HTV_LC_BURST_SHIFT;
+		pal = b == 1 || (b == 2 && (frame & 1) == 0) || (b == 3 && (frame & 1) == 1);
+		if(dp.colour_mode == HTV_PAL && pal && ((frame + line) & 1)) pal = -1;
+		const unsigned long long cw = dp.clut_width;
+		clut_off = (unsigned) (((unsigned long long) phase * ((unsigned long long) dp.lines * W % cw) + (unsigned long long) (line - 1) * W) % cw);
+	}
+	if(tid < 2 * UOFF)
+	{
+		const int j = tid < UOFF ? tid : W4 + tid;
+		su[j] = 0; sv[j] = 0;
+	}
+	const int x0 = tid * SPT;
+	const size_t at = (start ? (size_t) dt.comp_start + blockIdx.x : ((size_t) slot * dt.comp_phases + phase) * dp.lines + line - 1) * W + x0;
+	int val[SPT], uu[SPT], vv[SPT], cq[SPT] = { 0, 0, 0, 0 };
+	if(x0 < W)
+	{
+		raster_pic4(dp, dt, tmpl, al, ar, dt.tmpl_keep_any[tmpl], rgb, x0, val, uu, vv);
+		*reinterpret_cast<int4 *>(su + x0 + UOFF) = make_int4(uu[0], uu[1], uu[2], uu[3]);
+		*reinterpret_cast<int4 *>(sv + x0 + UOFF) = make_int4(vv[0], vv[1], vv[2], vv[3]);
+	}
+	if(pal)
+	{
+		__syncthreads();
+		// ---- chroma low-pass (saturating, int16), burst, subcarrier (ref video.c:3011-3040) ----
+		if(x0 < W)
+		{
+			int cu[SPT] = { 0, 0, 0, 0 }, cv[SPT] = { 0, 0, 0, 0 };
+			if(al < ar)
+			{
+				chroma_lp4(dp, su, sv, x0, cu, cv);
+				#pragma unroll
+				for(int k = 0; k < SPT; k++) { cu[k] = (int) (short) cu[k]; cv[k] = (int) (short) cv[k]; }
+			}
+			#pragma unroll
+			for(int k = 0; k < SPT; k++)
+			{
+				const int x = x0 + k;
+				if(x >= W) break;
+				if(x >= dp.burst_left && x < dp.burst_left + dp.burst_width)
+				{
+					const int w = dt.burst_win[x - dp.burst_left];
+					cu[k] = (dp.burst_i * w) >> 15;
+					cv[k] = (dp.burst_q * w) >> 15;
+				}
+				const htv_c16_t c = dt.clut[clut_off + x];
+				cq[k] = ((int) c.i * cv[k] * pal + (int) c.q * cu[k]) >> 15;
+				if(!dt.comp_q) val[k] += cq[k];
+			}
+		}
+	}
+	if(x0 >= W) return;
+	if((W & 3) == 0)                                                // at is a multiple of 4: one 8-byte store
+	{
+		*reinterpret_cast<uint2 *>(dt.comp + at) = make_uint2((val[0] & 0xFFFF) | (val[1] << 16), (val[2] & 0xFFFF) | (val[3] << 16));
+		if(dt.comp_q) *reinterpret_cast<uint2 *>(dt.comp_q + at) = make_uint2((cq[0] & 0xFFFF) | (cq[1] << 16), (cq[2] & 0xFFFF) | (cq[3] << 16));
+	}
+	else for(int k = 0; k < SPT; k++) if(x0 + k < W)
+	{
+		dt.comp[at + k] = (int16_t) val[k];
+		if(dt.comp_q) dt.comp_q[at + k] = (int16_t) cq[k];
+	}
 }
 
 // ---------------------------------------------------------------------------
@@ -2268,19 +2382,24 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 
 typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, int, int, int16_t *, const int16_t *, int, const int16_t *,
 	const int16_t *);
-struct KLine { KLineFn fn; int vf, hq, full, csat, maxt, minb, src, snd, wc, st; };
-#define KL_ENTRY(VF, HQ, FU, CS, T, SRC, SND, WC, ST) \
-	{ k_line<VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST>, VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST }
+// ps: the converted picture store and the subcarrier stage in k_line (encoders without a composite store); not part of
+// the name htv_line_kernel reports
+struct KLine { KLineFn fn; int vf, hq, full, csat, maxt, minb, src, snd, wc, st, ps; };
+#define KL_ENTRY_PS(VF, HQ, FU, CS, T, SRC, SND, WC, ST, PS) \
+	{ k_line<VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST, PS>, VF, HQ, FU, CS, T, KL_MINB(T), SRC, SND, WC, ST, PS }
+#define KL_ENTRY(VF, HQ, FU, CS, T, SRC, SND, WC, ST) KL_ENTRY_PS(VF, HQ, FU, CS, T, SRC, SND, WC, ST, false)
 // at each CTA size, the int16 store and the store converting to dp.sample_type at run time
-#define KL_MAXT(VF, HQ, FU, CS, SRC) \
-	KL_ENTRY(VF, HQ, FU, CS, 256, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 256, SRC, -1, 0, -1), \
-	KL_ENTRY(VF, HQ, FU, CS, 320, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 320, SRC, -1, 0, -1), \
-	KL_ENTRY(VF, HQ, FU, CS, 384, SRC, -1, 0, HTV_TYPE_INT16), KL_ENTRY(VF, HQ, FU, CS, 384, SRC, -1, 0, -1)
+#define KL_MAXT(VF, HQ, FU, CS, SRC, PS) \
+	KL_ENTRY_PS(VF, HQ, FU, CS, 256, SRC, -1, 0, HTV_TYPE_INT16, PS), KL_ENTRY_PS(VF, HQ, FU, CS, 256, SRC, -1, 0, -1, PS), \
+	KL_ENTRY_PS(VF, HQ, FU, CS, 320, SRC, -1, 0, HTV_TYPE_INT16, PS), KL_ENTRY_PS(VF, HQ, FU, CS, 320, SRC, -1, 0, -1, PS), \
+	KL_ENTRY_PS(VF, HQ, FU, CS, 384, SRC, -1, 0, HTV_TYPE_INT16, PS), KL_ENTRY_PS(VF, HQ, FU, CS, 384, SRC, -1, 0, -1, PS)
 // no video filter, a real low-pass, VSB
-#define KL_VF(FU, CS, SRC) KL_MAXT(false, false, FU, CS, SRC), KL_MAXT(true, false, FU, CS, SRC), KL_MAXT(true, true, FU, CS, SRC)
+#define KL_VF(FU, CS, SRC, PS) KL_MAXT(false, false, FU, CS, SRC, PS), KL_MAXT(true, false, FU, CS, SRC, PS), \
+	KL_MAXT(true, true, FU, CS, SRC, PS)
 static const KLine kl_tab[] = {
-	KL_VF(true, false, false), KL_VF(false, false, false), KL_VF(false, true, false),   // 128 | W, a partial last tile, CSAT
-	KL_VF(true, false, true), KL_VF(false, false, true),                                // SECAM's SRC form: 128 | W, partial
+	KL_VF(true, false, false, false), KL_VF(false, false, false, false), KL_VF(false, true, false, false),   // 128 | W, a partial last tile, CSAT
+	KL_VF(true, false, false, true), KL_VF(false, false, false, true), KL_VF(false, true, false, true),      // the same, PS
+	KL_VF(true, false, true, false), KL_VF(false, false, true, false),                  // SECAM's SRC form: 128 | W, partial
 	// PAL's VSB + FM + NICAM + complex output and W = 1024 (16 Msps) compiled in, storing int16 or int8 (the HackRF's format)
 	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT16),
 	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8),
@@ -2517,7 +2636,7 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	{
 		// the chroma low-pass cannot leave the int16 range when the sum of |taps| is at most 32768. The Gaussian taps are
 		// rounded one by one, so at about 1 % of sample rates they sum to 32769 .. 32771 (17.734475, 20.05 Msps: 32769),
-		// and those rates run the CSAT form. The saturation itself is k_picture's now, so the CSAT forms run the code of
+		// and those rates run the CSAT form. The saturation itself is k_compose's now, so the CSAT forms run the code of
 		// the partial-tile form; they, and the partial-tile form for CSAT rates where 128 divides W, stay only because the
 		// instantiation names htv_line_kernel reports are pinned by the tests
 		long long sum = 0;
@@ -2526,11 +2645,13 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 		// the common case (128 | W, a chroma filter that cannot overflow) has its own instantiation, everything else the
 		// general one; within it VSB + FM + NICAM + complex output at W = 1024 (PAL-I, B/G at 16 Msps) one with those
 		// sound stages and the width compiled in, storing int16 or int8; other sample types run the general form
-		const bool fixed = hq && !csat && W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !sw.kl_general &&
+		// encoders whose subcarrier does not repeat within 4 frames have no composite store: the PS forms
+		const int ps = t->comp_phases == 0;
+		const bool fixed = !ps && hq && !csat && W == 1024 && kl_snd_mask(dp) == KL_SND_FM_NICAM && !sw.kl_general &&
 			(type == HTV_TYPE_INT16 || type == HTV_TYPE_INT8);
 		p->kl = kfind(kl_tab, miss, [&](const KLine &k) {
 			return(k.vf == vf && k.hq == hq && k.full == (full && !csat) && k.csat == csat && k.maxt == maxt && !k.src &&
-				k.snd == (fixed ? KL_SND_FM_NICAM : -1) && k.wc == (fixed ? W : 0) && k.st == (fixed ? type : kst)); });
+				k.snd == (fixed ? KL_SND_FM_NICAM : -1) && k.wc == (fixed ? W : 0) && k.st == (fixed ? type : kst) && k.ps == ps); });
 		break;
 	}
 	case PATH_SEC_LINE:
@@ -2585,8 +2706,8 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	{
 		kl_name(kl, sizeof(kl), *p->kl, type, dp.s_video);
 		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
-		// S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
-		if(dp.s_video && p->path == PATH_LINE) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
+		// PS forms with S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
+		if(dp.s_video && p->kl->ps) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
 	}
 	if(p->path == PATH_LINE) snprintf(p->kname, sizeof(p->kname), "%s", kl);
 	else if(p->ks) snprintf(p->kname, sizeof(p->kname), "%s<FULL=%d,MAXT=%d> + %s", rname, p->ks->full, p->ks->maxt, kl);
@@ -2631,12 +2752,12 @@ extern "C" int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, 
 
 // An encoder's side streams and events, in the one list htv_dev_create creates and htv_dev_destroy destroys. ev0 and
 // ev1 time the last modulator launch (htv_dev_last_line_ms); every other event only orders work, without timing.
-struct DevSync { cudaStream_t *stream[5]; cudaEvent_t *timed[2]; cudaEvent_t *event[11]; };
+struct DevSync { cudaStream_t *stream[5]; cudaEvent_t *timed[2]; cudaEvent_t *event[10]; };
 static DevSync dev_sync(htv_dev_t *d)
 {
 	return(DevSync{ { &d->side, &d->side2, &d->side3, &d->up, &d->pic }, { &d->ev0, &d->ev1 },
 		{ &d->ev_nic, &d->ev_up, &d->ev_chunk[0], &d->ev_chunk[1], &d->ev_in, &d->ev_kl[0], &d->ev_kl[1], &d->ev_r2, &d->ev_audio,
-		  &d->ev_copied, &d->ev_pic } });
+		  &d->ev_pic } });
 }
 
 // htv_dev_create's way out: the message, and everything allocated so far freed
@@ -2721,9 +2842,15 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	dt.frame_map = d->d_frame_map;
 	if(p.path == PATH_LINE)
 	{
-		// the converted picture store (k_picture): a row per source row of every slot and of the black slot, which also
-		// holds the lines with a picture area and no source row; (max_slots + 1) x pic_nrows x W x 6 bytes (60 MB for
-		// PAL at 16 Msps)
+		d->ev_slot = (cudaEvent_t *) calloc((size_t) d->max_slots, sizeof(cudaEvent_t));
+		if(!d->ev_slot) return(create_fail(d, err, errlen, "out of memory"));
+		for(int i = 0; i < d->max_slots; i++)
+			if(cudaEventCreateWithFlags(&d->ev_slot[i], cudaEventDisableTiming) != cudaSuccess) return(create_fail(d, err, errlen, "event creation failed"));
+	}
+	if(p.path == PATH_LINE && !t->comp_phases)
+	{
+		// the converted picture store (k_picture) of the PS forms: a row per source row of every slot and of the black
+		// slot, which also holds the lines with a picture area and no source row; (max_slots + 1) x pic_nrows x W x 6 bytes
 		dt.pic_rows = (const int4 *) dev_copy(d, t->pic_rows, sizeof(int32_t) * 4 * t->pic_nrows);
 		dt.line_row = (const int32_t *) dev_copy(d, t->line_row, sizeof(int32_t) * (dp.lines + 1));
 		dt.pic_nrows = t->pic_nrows;
@@ -2731,6 +2858,23 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		const size_t n = (size_t) (d->max_slots + 1) * t->pic_nrows * dp.W;
 		dt.pic_val = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
 		if(dp.colour_mode != HTV_MONOCHROME) dt.pic_cuv = (uint32_t *) dev_zero(d, sizeof(uint32_t) * n);
+	}
+	if(p.path == PATH_LINE && t->comp_phases)
+	{
+		// the composite store (k_compose): every line of every slot and of the black slot at each colour-frame phase, and
+		// the two stream-start rows; ((max_slots + 1) x comp_phases x lines + 2) x W x 2 bytes, twice with S-Video (87 MB
+		// for PAL at 16 Msps). Stream line 0 shares its row with every encoder start: it must have no picture area.
+		if(t->codes[1] & (HTV_LC_LEFT_ACTIVE | HTV_LC_RIGHT_ACTIVE))
+			return(create_fail(d, err, errlen, "line 1 of the frame has a picture area: not on the fused line kernel"));
+		dt.comp_phases = t->comp_phases;
+		dt.comp_black = d->max_slots;
+		dt.comp_start = (int64_t) (d->max_slots + 1) * dt.comp_phases * dp.lines;
+		const size_t n = (size_t) (dt.comp_start + 2) * dp.W;
+		if(n >= (size_t) INT32_MAX) return(create_fail(d, err, errlen, "composite store of %zu samples: more than k_line addresses", n));
+		d->comp_valid = (uint8_t *) calloc((size_t) d->max_slots, 1);
+		if(!d->comp_valid) return(create_fail(d, err, errlen, "out of memory"));
+		dt.comp = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
+		if(dp.s_video) dt.comp_q = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
 	}
 	dt.pcm = d->d_pcm;
 	if(dp.have_fm)
@@ -2852,8 +2996,13 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	}
 	if(d->alloc_failed) return(create_fail(d, err, errlen, "device allocation failed"));
 	if(!plan_attributes(p, err, errlen)) { htv_dev_destroy(d); return(NULL); }
-	// the black slot, once: every row from zero RGB, behind the RGB -> YUV table on the default stream
+	// the black slot (at every phase) and the stream-start rows, once, behind the RGB -> YUV table on the default stream
 	if(dt.pic_val) k_picture<<<dim3(dt.pic_nrows, 1), p.line_threads, p.raster_smem>>>(dp, dt, dt.pic_black);
+	if(dt.comp)
+	{
+		for(int ph = 0; ph < t->comp_phases; ph++) k_compose<<<dp.lines, p.line_threads, p.raster_smem>>>(dp, dt, dt.comp_black, ph, 0);
+		k_compose<<<2, p.line_threads, p.raster_smem>>>(dp, dt, dt.comp_black, 0, 1);
+	}
 	const DevSync sy = dev_sync(d);
 	bool made = true;
 	for(cudaStream_t *s : sy.stream) made &= cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
@@ -2885,6 +3034,9 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	for(cudaStream_t *s : sy.stream) if(*s) cudaStreamDestroy(*s);
 	for(cudaEvent_t *e : sy.timed) if(*e) cudaEventDestroy(*e);
 	for(cudaEvent_t *e : sy.event) if(*e) cudaEventDestroy(*e);
+	free(d->comp_valid);
+	if(d->ev_slot) for(int i = 0; i < d->max_slots; i++) if(d->ev_slot[i]) cudaEventDestroy(d->ev_slot[i]);
+	free(d->ev_slot);
 	free(d);
 }
 
@@ -2902,11 +3054,6 @@ extern "C" int htv_dev_uploads_end(htv_dev_t *d, void *stream)
 	DevGuard guard(d->device);
 	CK(cudaEventRecord(d->ev_up, d->up));
 	CK(cudaStreamWaitEvent((cudaStream_t) stream, d->ev_up, 0));
-	if(d->dt.pic_val)
-	{
-		CK(cudaEventRecord(d->ev_pic, d->pic));
-		CK(cudaStreamWaitEvent((cudaStream_t) stream, d->ev_pic, 0));
-	}
 	return(HTV_OK);
 }
 
@@ -2953,20 +3100,25 @@ extern "C" int htv_dev_set_overlays(htv_dev_t *d, int n, const long long *line, 
 	return(HTV_OK);
 }
 
-// The converted picture store of slots slot .. slot + count - 1, right behind their copy on `st` (fused line kernel only).
-// Its slots are under the RGB slots' protection: the host cycles 16 slots and brings at most 7 new pictures per call
-// (htv_host.c), and the uploads of call c wait for call c - 2's kernels (htv_dev_uploads_begin), which the conversion
-// waits for through its copy. It runs on a stream of its own, so that the next copies on the upload stream go on
-// beside it; htv_dev_uploads_end makes the caller's stream wait for it (ev_pic) as for the copies (ev_up). Call c + 1's
-// copies touch none of the RGB slots call c converts: they are the next 7 of the 16.
-static int convert_pictures(htv_dev_t *d, int slot, int count, cudaStream_t st)
+// A new picture in slots slot .. slot + count - 1, copied on `st`. The conversions run on the pic stream, each behind its
+// slot's copy, so that the next copies on the upload stream go on beside them; the caller's stream waits for them
+// (ev_pic) only when there were any. The converted picture store (PS forms) converts the picture here, the composite
+// store marks all phases of the slot stale for htv_dev_set_frame_map. Their slots are under the RGB slots' protection:
+// the host cycles 16 slots and brings at most 7 new pictures per call (htv_host.c), and the uploads of call c wait for
+// call c - 2's kernels (htv_dev_uploads_begin), which waited for their conversions.
+static int slots_uploaded(htv_dev_t *d, int slot, int count, cudaStream_t st)
 {
-	if(!d->dt.pic_val) return(HTV_OK);
-	CK(cudaEventRecord(d->ev_copied, st));
-	CK(cudaStreamWaitEvent(d->pic, d->ev_copied, 0));
-	k_picture<<<dim3(d->dp.active_lines, count), d->plan.line_threads, d->plan.raster_smem, d->pic>>>(d->dp, d->dt, slot);
-	d->launches++;
-	CK(cudaGetLastError());
+	if(!d->ev_slot) return(HTV_OK);
+	for(int i = slot; i < slot + count; i++) CK(cudaEventRecord(d->ev_slot[i], st));
+	if(d->comp_valid) memset(d->comp_valid + slot, 0, (size_t) count);
+	if(d->dt.pic_val)
+	{
+		CK(cudaStreamWaitEvent(d->pic, d->ev_slot[slot], 0));
+		k_picture<<<dim3(d->dp.active_lines, count), d->plan.line_threads, d->plan.raster_smem, d->pic>>>(d->dp, d->dt, slot);
+		d->launches++;
+		CK(cudaGetLastError());
+		d->pic_pending = 1;
+	}
 	return(HTV_OK);
 }
 
@@ -2976,23 +3128,50 @@ extern "C" int htv_dev_upload_frame(htv_dev_t *d, int slot, const uint32_t *rgb,
 	if(slot < 0 || slot >= d->max_slots) return(HTV_ERROR);
 	CK(cudaMemcpyAsync(d->d_frames + (size_t) slot * d->frame_pixels, rgb, d->frame_pixels * 4,
 		cudaMemcpyHostToDevice, (cudaStream_t) stream));
-	return(convert_pictures(d, slot, 1, (cudaStream_t) stream));
+	return(slots_uploaded(d, slot, 1, (cudaStream_t) stream));
 }
 
-// `count` pictures, contiguous in host memory, into `count` consecutive slots: one copy
+// `count` pictures, contiguous in host memory, into `count` consecutive slots
 extern "C" int htv_dev_upload_frames(htv_dev_t *d, int slot, int count, const uint32_t *rgb, void *stream)
 {
 	DevGuard guard(d->device);
 	if(slot < 0 || count < 1 || slot + count > d->max_slots) return(HTV_ERROR);
-	// with the picture store, the last picture goes up in a copy of its own: the others are converted while it is copied,
-	// so that one picture's conversion, not the run's, stands between the copies and the line kernel that waits for both
-	const int head = d->dt.pic_val && count > 1 ? count - 1 : count;
+	// with a store, the last picture goes up in a copy of its own: the others can be converted while it is copied, so
+	// that one picture's conversion, not the run's, stands between the copies and the line kernel
+	const int head = d->ev_slot && count > 1 ? count - 1 : count;
 	for(int at = 0, n = head; at < count; at += n, n = count - at)
 	{
 		CK(cudaMemcpyAsync(d->d_frames + (size_t) (slot + at) * d->frame_pixels, rgb + (size_t) at * d->frame_pixels,
 			d->frame_pixels * 4 * (size_t) n, cudaMemcpyHostToDevice, (cudaStream_t) stream));
-		const int r = convert_pictures(d, slot + at, n, (cudaStream_t) stream);
+		const int r = slots_uploaded(d, slot + at, n, (cudaStream_t) stream);
 		if(r != HTV_OK) return(r);
+	}
+	return(HTV_OK);
+}
+
+// The composite rows the frames of this call show and no conversion has filled since their slot's picture came up:
+// (slot, frame mod comp_phases) for each frame with a picture (the black slot's are converted at htv_dev_create). A
+// (slot, phase) entry is written only when its slot has just been uploaded, or when no line has read that phase since,
+// so no line kernel reads it meanwhile. Then the caller's stream waits for this call's conversions, if there were any.
+static int convert_frames(htv_dev_t *d, const int32_t *slot_of_frame, int n, int64_t first_frame, cudaStream_t stream)
+{
+	const int P = d->dt.comp_phases;
+	for(int i = 0; d->comp_valid && i < n; i++)
+	{
+		const int s = slot_of_frame[i], ph = (int) ((first_frame + i) % P);
+		if(s < 0 || s >= d->max_slots || (d->comp_valid[s] >> ph & 1)) continue;
+		CK(cudaStreamWaitEvent(d->pic, d->ev_slot[s], 0));
+		k_compose<<<d->dp.lines, d->plan.line_threads, d->plan.raster_smem, d->pic>>>(d->dp, d->dt, s, ph, 0);
+		d->launches++;
+		CK(cudaGetLastError());
+		d->comp_valid[s] |= (uint8_t) (1u << ph);
+		d->pic_pending = 1;
+	}
+	if(d->pic_pending)
+	{
+		CK(cudaEventRecord(d->ev_pic, d->pic));
+		CK(cudaStreamWaitEvent(stream, d->ev_pic, 0));
+		d->pic_pending = 0;
 	}
 	return(HTV_OK);
 }
@@ -3025,7 +3204,7 @@ extern "C" int htv_dev_set_frame_map(htv_dev_t *d, const int32_t *slot_of_frame,
 	}
 	d->dt.frame_map_first = first_frame;
 	d->dt.frame_map_len = n;
-	return(HTV_OK);
+	return(convert_frames(d, slot_of_frame, n, first_frame, (cudaStream_t) stream));
 }
 
 extern "C" int htv_dev_upload_audio(htv_dev_t *d, int64_t j0, const int16_t *pcm, size_t npairs, void *stream)

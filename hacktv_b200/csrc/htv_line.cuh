@@ -4,10 +4,10 @@
 // the picture in HBM and the int16 IQ in HBM - raster, chroma, video filter, sound carriers, mixers -
 // without the composite signal ever leaving the SM:
 //
-//   R1  the line's row of the converted picture store: template (blank + sync pulses) + Y, and U, V after the chroma
-//       low-pass, converted once per picture when it arrived (k_picture, ref video.c:2864-2992, fir.c:357-375)
-//   R2  burst, subcarrier mix (ref video.c:3011-3040), VBI overlay; the finished composite line goes into a 4-row ring
-//       of byte planes in shared memory
+//   R1  the line's row of the composite store: template (blank + sync pulses) + Y + the low-passed chroma on the
+//       subcarrier + burst, converted once per picture and colour-frame phase (k_compose, ref video.c:2864-3040,
+//       fir.c:357-375)
+//   R2  VBI overlay; the finished composite line goes into a 4-row ring of byte planes in shared memory
 //   M   51-tap VSB / low-pass video filter on the tensor cores (ref video.c:3235-3248, fir.c:564-615),
 //       FM / AM / NICAM sound carriers (ref video.c:3261-3450, nicam728.c:342-411), IQ swap, offset
 //       mixer (ref video.c:3466-3515), channel combiner, store.
@@ -100,11 +100,11 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 
 // VF: a video filter is on (composite ring + tensor-core FIR); HASQ: it has Q taps (VSB); FULL: 128 | W (no
 // partial tile: the x < W tests fold away); CSAT: the chroma low-pass can leave the int16 range (sum of |taps| > 32768),
-// which k_picture's saturating low-pass handles when it fills the store: the CSAT forms run the same code as the others
+// which k_compose's saturating low-pass handles when it fills the store: the CSAT forms run the same code as the others
 //
 // Per iteration q (one scan line) a CTA runs
-//   R2(q)   burst, subcarrier, VBI overlay on the values fetched earlier, composite row q mod 4  | __syncthreads
-//   R1(q+1) the converted row of the NEXT line (values, and filtered U / V on colour lines) is loaded here ...
+//   R2(q)   VBI overlay on the values fetched earlier, composite row q mod 4                  | __syncthreads
+//   R1(q+1) the composite row of the NEXT line is loaded here ...
 //   M(q-1)  ... and arrive while line q - 1 (whose right-hand halo R2(q) has just written) is filtered (mma),
 //           gets its sound carriers and is stored.
 // The line descriptors (LineR2 of q + 1, LineA2 of q - 1) come in by cp.async at the top of the iteration.
@@ -117,11 +117,16 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 // WC: the line width compiled in (0: dp.W), so that the shared-memory row and plane offsets become immediates
 // ST: the output sample type compiled into the store (HTV_TYPE_INT16: the int16 store), -1: dp.sample_type at run time
 //
-// S-Video (KL_SV, dp.s_video; ref video.c:3031-3040, 3206-3228): the subcarrier term of R2 goes to Q instead of I, and the
-// video filter runs on I only, so Q of the stored line is that line's own chroma. R2 parks it in a two-row ring in shared
-// memory at the lane's own slots (row q & 1), M takes it back for mrow: no other thread touches the slots, so no barrier
-// orders them, and nothing stays live in registers across the loop. SRC: the chain wrote Q into its own plane, `srcq`.
-template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16>
+// PS: encoders whose colour subcarrier does not repeat within 4 frames (htv_tables.c comp_phases = 0) have no composite
+// store. Their R1 reads the converted picture store instead - template + Y and, on colour lines, U | V << 16 after the
+// chroma low-pass, converted once per picture (k_picture) - and R2 adds burst and subcarrier (ref video.c:3011-3040).
+//
+// S-Video (KL_SV, dp.s_video; ref video.c:3031-3040, 3206-3228): the subcarrier term goes to Q instead of I, and the
+// video filter runs on I only, so Q of the stored line is that line's own chroma. k_compose wrote it into the store's
+// chroma plane (dt.comp_q), which M reads at the row of mrow; SRC: the chain wrote Q into its own plane, `srcq`; PS: R2
+// parks it in a two-row ring in shared memory at the lane's own slots (row q & 1), which M takes back for mrow.
+template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16,
+	bool PS = false>
 __global__ void __launch_bounds__(MAXT, MINB)
 k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap,
 	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr, const int16_t *srcq = nullptr)
@@ -129,7 +134,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	const int W = WC ? WC : dp.W;
 	const int RB = kl_row_bytes(W);
-	// descriptors x2 | [row 0..3][hi, lo] composite planes | FIR taps | NICAM pulse | S-Video chroma [row 0..1][j][thread]
+	// descriptors x2 | [row 0..3][hi, lo] composite planes | FIR taps | NICAM pulse | PS, S-Video: chroma [row 0..1][j][thread]
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
 	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + 2);
 	unsigned char *rows = reinterpret_cast<unsigned char *>(slr + 2);
@@ -158,21 +163,21 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	if(!SRC && tid < 4) reinterpret_cast<int4 *>(slr + (q0 & 1))[tid] = __ldg(reinterpret_cast<const int4 *>(lrp + q0 + 1) + tid);
 	__syncthreads();
 
-	// the span the chroma low-pass reaches (taps <= 17: 8 samples either side of the picture); the store is zero outside
+	// PS: the span the chroma low-pass reaches (taps <= 17: 8 samples either side of the picture); the store is zero outside
 	const bool in_chroma = xb + 24 >= dp.active_left - 8 && xb < dp.active_left + dp.active_width + 8;
 	const bool in_burst = xb + 24 >= dp.burst_left && xb < dp.burst_left + dp.burst_width;
 	const int fo0 = mf_b_offset(nt, 0, lane);
 	constexpr int NA16 = (int) (sizeof(LineA2) / 16);
 
-	// loads of line q issued one phase early: line values (int16 x 4) and, on colour lines, filtered U | V << 16 (x 4)
+	// loads of line q issued one phase early: the line's composite row (int16 x 4); PS: line values (int16 x 4) and, on
+	// colour lines, filtered U | V << 16 (x 4)
 	int tm[4];
 	unsigned px[4];
 	#define KL_R1(QQ) do { \
-		if(SRC) \
+		if(!PS) \
 		{ \
-			const int16_t *sp_ = src + (size_t) ((QQ) + 2) * W + xb; \
-			_Pragma("unroll") for(int j = 0; j < 4; j++) tm[j] = (FULL || xb + 8 * j < W) ? (int) __ldg(sp_ + 8 * j) : 0; \
-			px[0] = px[1] = px[2] = px[3] = 0u; \
+			const int16_t *tp_ = SRC ? src + (size_t) ((QQ) + 2) * W + xb : dt.comp + slr[(QQ) & 1].pic + xb; \
+			_Pragma("unroll") for(int j = 0; j < 4; j++) tm[j] = (FULL || xb + 8 * j < W) ? (int) __ldg(tp_ + 8 * j) : 0; \
 			break; \
 		} \
 		const LineR2 &ln = slr[(QQ) & 1]; \
@@ -187,6 +192,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		else { px[0] = px[1] = px[2] = px[3] = 0u; } \
 	} while(0)
 	KL_R1(q0);
+	int ppic = 0;                                                           // S-Video: the row of line q - 1 (< 2^31, htv_dev_create)
 
 	int r4 = q0 & 3;                                                        // ring row of line q
 	for(int q = q0; q <= q1; q++, r4 = (r4 + 1) & 3)
@@ -201,13 +207,15 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			for(int i = (int) blockDim.x - 4 + tid; i < NA16; i += blockDim.x)
 				kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + i, reinterpret_cast<const int4 *>(lap + mrow) + i);
 
-		// ---- R2: burst, subcarrier, VBI overlay of line q ---------------------------
+		// ---- R2: (PS: burst, subcarrier,) VBI overlay of line q ---------------------
 		const LineR2 &li = slr[q & 1];
-		const int li_pal = SRC ? 0 : li.pal;
 		int val[4] = { tm[0], tm[1], tm[2], tm[3] };
-		int cq[4] = { 0, 0, 0, 0 };                                         // S-Video: the chroma of line q
-		if(li_pal)
+		int mpic = 0;                                                       // S-Video: the row of the line modulated below
+		if(!SRC && !PS && sv) { mpic = VF ? ppic : (int) li.pic; ppic = (int) li.pic; }
+		int cq[4] = { 0, 0, 0, 0 };                                         // PS, S-Video: the chroma of line q
+		if(PS && li.pal)
 		{
+			const int li_pal = li.pal;
 			short2 cl[4];
 			{
 				const htv_c16_t *cp = dt.clut + li.clut_off + xb;
@@ -242,7 +250,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 				for(int j = 0; j < 4; j++) val[j] += ((int) cl[j].x * cv[j] * li_pal + (int) cl[j].y * cu[j]) >> 15;
 			}
 		}
-		if(!SRC && sv)
+		if(PS && sv)
 		{
 			#pragma unroll
 			for(int j = 0; j < 4; j++) svq[((q & 1) * 4 + j) * blockDim.x + tid] = (short) cq[j];
@@ -338,12 +346,12 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			if(sv)
 			{
 				// Q = the chroma of line mrow (the video filter leaves it alone)
-				const int16_t *qp = srcq + (size_t) (mrow + 2) * W + xb;
+				const int16_t *qp = (SRC ? srcq + (size_t) (mrow + 2) * W : PS ? srcq : dt.comp_q + mpic) + xb;
 				#pragma unroll
 				for(int j = 0; j < 4; j++)
 				{
-					if(SRC) oq[j] += (FULL || xb + 8 * j < W) ? (int) __ldg(qp + 8 * j) : 0;
-					else oq[j] += svq[((mrow & 1) * 4 + j) * blockDim.x + tid];
+					if(PS) oq[j] += svq[((mrow & 1) * 4 + j) * blockDim.x + tid];
+					else oq[j] += (FULL || xb + 8 * j < W) ? (int) __ldg(qp + 8 * j) : 0;
 				}
 			}
 			const LineA2 *la = sla + (mrow & 1);

@@ -297,7 +297,7 @@ static int build_templates(struct htv_tables_t *t)
 	return(0);
 }
 
-/* ---- picture rows (converted picture store) ------------------------------ *
+/* ---- picture rows (converted picture store of the encoders without a composite store, comp_phases = 0) ---- *
  * Which line of the frame shows each source picture row, with that line's picture geometry, so that a picture can be
  * converted (RGB -> Y, U, V, chroma low-pass, the line template) row by row when it arrives, not line by line on every
  * frame that shows it. The picture area [al, ar) of a line as the raster descriptors have it (k_line_desc_r): the whole
@@ -536,6 +536,20 @@ htv_tables_t *htv_tables_create(const htv_config_t *conf, unsigned int sample_ra
 				return(NULL);
 			}
 		}
+	}
+
+	/* colour-frame phases of the composite store: a line's subcarrier offset (L W mod clut_width), V-switch and burst
+	 * code repeat after this many frames - the period of lines W mod clut_width, and 2 for the frame parity the
+	 * V-switch and burst codes take. 4 for PAL, PAL-N and PAL-M where the line is a whole number of samples, 2 for NTSC,
+	 * 1 without colour; 0: more than 4 (a carrier that is no quarter-line multiple of the line rate, as PAL-60's, or a
+	 * rounded line width): those encoders keep the converted picture store and the subcarrier stage in k_line. */
+	t->comp_phases = 1;
+	if(c->colour_mode == HTV_PAL || c->colour_mode == HTV_NTSC)
+	{
+		const int64_t cw = dp->clut_width, step = (int64_t) ((uint64_t) dp->lines * (uint64_t) dp->W % (uint64_t) cw);
+		const int64_t p = step ? cw / gcd64(cw, step) : 1;
+		t->comp_phases = p > 4 ? 0 : (int) (p % 2 == 0 ? p : 2 * p);
+		if(t->comp_phases > 4) t->comp_phases = 0;
 	}
 
 	if(c->burst_level > 0 || c->colour_mode == HTV_SECAM)
@@ -987,6 +1001,11 @@ const int32_t *htv_tables_get(htv_tables_t *t, const char *name, int *count)
 	}
 	if(!strcmp(name, "pic_rows")) return(view32(t, t->pic_rows, 4 * t->pic_nrows, count));
 	if(!strcmp(name, "line_row")) return(view32(t, t->line_row, dp->lines + 1, count));
+	if(!strcmp(name, "comp_phases"))
+	{
+		tmp[0] = t->comp_phases; tmp[1] = (int32_t) dp->clut_width;
+		return(view32(t, tmp, 2, count));
+	}
 	if(!strcmp(name, "codes"))
 	{
 		int i;

@@ -1,6 +1,7 @@
-"""What a live source pays for the converted picture store: the time of k_picture per picture (one conversion per
-uploaded picture) beside the host-to-device copy of the same picture, from torch.profiler over a run with a new picture
-every frame. PAL-I at 16 Msps with the video filter, as bench.py's workload. Prints one JSON line.
+"""What a live source pays for the composite store: the time of k_compose per (picture, colour-frame phase) conversion
+beside the host-to-device copy of the same picture, from torch.profiler over a run with a new picture every frame (one
+conversion per picture: the phase of the frame that shows it). PAL-I at 16 Msps with the video filter, as bench.py's
+workload. Prints one JSON line.
     python tools/picture_time.py [frames]"""
 import json
 import os
@@ -33,15 +34,16 @@ def main():
     for e in prof.events():
         if e.device_type != torch.autograd.DeviceType.CUDA:
             continue
-        if "k_picture" in e.name:
+        if "k_compose" in e.name:
             conv.append(e.device_time)
         elif "Memcpy HtoD" in e.name and e.device_time > 50:
             copy.append(e.device_time)
     enc.close()
     pic_bytes = enc.active_lines * enc.active_width * 4
-    # consecutive pictures go up as one copy and are converted by one launch (htv_host.c), so count per picture
+    # consecutive pictures go up as one copy (htv_host.c), so count per picture
     n = 64 * (frames // 64)
-    print(json.dumps({"pictures": n, "k_picture_launches": len(conv), "k_picture_us_per_picture": float(np.sum(conv)) / n,
+    print(json.dumps({"pictures": n, "k_compose_launches": len(conv), "k_compose_us_per_conversion": float(np.sum(conv)) / max(len(conv), 1),
+                      "k_compose_us_per_picture": float(np.sum(conv)) / n,
                       "htod_copies": len(copy), "htod_us_per_picture": float(np.sum(copy)) / n, "picture_bytes": pic_bytes,
                       "gpu": torch.cuda.get_device_name(0)}))
 
