@@ -40,6 +40,7 @@ struct htv_t {
 	/* video frames */
 	int64_t cur_frame;            /* 0-based index of the last frame pulled, -1 none */
 	int cur_slot;                 /* its slot, -1 = no picture (black) */
+	int prev_slot;                /* the slot of frame cur_frame - 1 */
 	uint64_t cur_serial;
 	int have_serial;
 	int next_slot;
@@ -163,6 +164,7 @@ int htv_init_on(htv_t **out, int device, unsigned int sample_rate, unsigned int 
 	s->bps = htv_st_bytes(s->type, s->complex);
 	s->cur_frame = -1;
 	s->cur_slot = -1;
+	s->prev_slot = -1;
 	s->av.width = s->rtab->dp.active_width;
 	s->av.height = s->rtab->dp.active_lines;
 	s->zeros = htv_dev_alloc_pinned(65536 * 2 * sizeof(int16_t));    /* pinned: uploads stay asynchronous */
@@ -466,7 +468,11 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 	int n = *pn, nnew = 0;
 	const htv_dparams_t *dp = &s->tab->dp, *rdp = &s->rtab->dp;
 	const int64_t L0 = s->next_line;
-	const int64_t f0 = L0 / s->lines, f1 = (L0 + n - 1) / s->lines;
+	/* the frame map starts at the frame of line L0 - 2: lines L0 - 2 .. L0 - 1 are rasterised again as the left
+	 * neighbours of this launch (below), and where L0 opens a frame they are lines of the previous frame, with its
+	 * picture (the progressive 525-line raster shows a source row on its last line, and the video filter reaches back
+	 * into it from line 1) */
+	const int64_t fm = (L0 >= 2 ? L0 - 2 : 0) / s->lines, f0 = L0 / s->lines, f1 = (L0 + n - 1) / s->lines;
 	int32_t map[4096];
 	int64_t f;
 	int r, nmap = 0, run_n = 0, run_slot = 0;
@@ -474,7 +480,11 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 	const size_t fpix = (size_t) rdp->active_width * rdp->active_lines;
 	void *up, *rup;
 
-	if(f1 - f0 + 1 > 4096) return(HTV_ERROR);
+	if(f1 - fm + 1 > 4096) return(HTV_ERROR);
+	/* frame f0 - 1 was pulled by the previous call, which showed its picture: that call's last slot, or the one before
+	 * it where that call also pulled frame f0. Its slot is not reused before this launch has run (the slots cycle
+	 * through 16 and a call brings at most MAX_NEW_FRAMES), and its phase of the composite store is already converted */
+	if(fm < f0) map[nmap++] = s->cur_frame == f0 ? s->prev_slot : s->cur_slot;
 
 	/* pictures and PCM go up on the encoder's own upload stream, ahead of the kernels queued on
 	 * `stream` for the previous chunk and beside the caller's device-to-host copies */
@@ -506,6 +516,7 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 				break;
 			}
 			memset(&fr, 0, sizeof(fr));
+			s->prev_slot = s->cur_slot;
 			s->cur_frame = f;
 			if(s->av.read_video && s->av.read_video(s->av.ctx, &fr) == HTV_OK && fr.framebuffer)
 			{
@@ -566,7 +577,7 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 		if(r != HTV_OK) return(r);
 	}
 
-	r = htv_dev_set_frame_map(s->rdev, map, nmap, f0, stream);
+	r = htv_dev_set_frame_map(s->rdev, map, nmap, fm, stream);
 	if(r != HTV_OK) return(r);
 
 	if(dp->have_fm || dp->have_am || dp->have_nicam)
