@@ -617,12 +617,15 @@ static int max_chunk_lines(const htv_t *s)
 
 static int render_any(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, int add, void *cuda_stream)
 {
-	int done = 0, r, cap;
+	int done = 0, r, cap, align;
 	if(!s || nlines < 0 || !d_out) return(HTV_ERROR);
-	/* the kernels write (and, for htv_render_add, read) d_out with 128-bit accesses */
-	if(((uintptr_t) d_out & 15) != 0)
+	/* the widest access the store makes to d_out (and htv_render_add's combiner from it, htv_dev_out_align): four int16
+	 * samples in the split and FM-video modulators where 4 | W, else one sample. The sub-batches start whole lines in,
+	 * which keeps it */
+	align = htv_dev_out_align(s->dev);
+	if(((uintptr_t) d_out & (uintptr_t) (align - 1)) != 0)
 	{
-		fprintf(stderr, "hacktv_b200: the output buffer must be 16-byte aligned\n");
+		fprintf(stderr, "hacktv_b200: the output buffer must be %d-byte aligned\n", align);
 		return(HTV_ERROR);
 	}
 	cap = max_chunk_lines(s);

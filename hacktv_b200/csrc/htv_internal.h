@@ -191,6 +191,8 @@ extern float htv_dev_event_elapsed(void *e0, void *e1);
 extern int htv_dev_mix_add(int16_t *d_acc, const int16_t *d_in, size_t nvalues, void *stream);
 /* the kernels of the new type's stores (before the first rendered line); HTV_ERROR with a message on stderr */
 extern int htv_dev_set_sample_type(htv_dev_t *d, int type);
+/* the alignment htv_render / htv_render_add need of d_out (bytes): the widest access of the plan's store and combiner */
+extern int htv_dev_out_align(const htv_dev_t *d);
 /* the name htv_line_kernel would report for an encoder of these tables writing this sample type, under the switches
  * (HTV_PATH, HTV_FIR, HTV_KL) in the environment; the kernel selection alone, without a CUDA call (CPU tests) */
 extern int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, char *name, size_t len);

@@ -3642,6 +3642,16 @@ extern "C" int htv_dev_set_sample_type(htv_dev_t *d, int type)
 	return(HTV_OK);
 }
 
+// The alignment htv_render and htv_render_add need of d_out: the widest access the plan's store and channel combiner make
+// there. mod_store moves four int16 samples at a time where 4 | W (16 bytes complex, 8 real); every other store - k_line's
+// (kl_post_store), mod_store's per-sample branch and the typed stores - moves one sample, I and Q together
+extern "C" int htv_dev_out_align(const htv_dev_t *d)
+{
+	const htv_dparams_t &dp = d->dp;
+	if(d->plan.kl || dp.sample_type != HTV_TYPE_INT16 || (dp.W & 3)) return(htv_st_bytes(dp.sample_type, dp.complex_out));
+	return(dp.complex_out ? 16 : 8);
+}
+
 // htv_convert: dst[i] = the `type` form of src[i] (htv_sample_type.h), eight values per thread and step: one 16-byte
 // load, one store of 8, 16 or 32 bytes
 template<int T>

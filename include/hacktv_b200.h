@@ -264,8 +264,12 @@ extern int htv_set_prefetch(htv_t *s, int on);
  * htv_render_host: `h_out` is HOST memory; the call uploads what the batch
  *   needs, renders, copies the result back and returns when it is there.
  * Both return HTV_OK or an error; *nsamples (may be NULL) receives the number
- * of samples produced. `d_out` must be 16-byte aligned (the kernels store, and htv_render_add
- * also loads, 128 bits at a time); a misaligned pointer is refused with HTV_ERROR. Output layout is what the reference's file sink writes
+ * of samples produced. `d_out` must be aligned to the widest access the encoder's store (and
+ * htv_render_add's loads) make: 16 bytes where the split and FM-video modulators store four
+ * complex int16 samples at once (4 divides the line width), 8 for four real ones, otherwise one
+ * sample (htv_bytes_per_sample). A pointer a whole number of lines into a 16-byte aligned buffer
+ * always qualifies - the reference's two-channel alignment, one line in, at any width. A
+ * misaligned pointer is refused with HTV_ERROR. Output layout is what the reference's file sink writes
  * (rf_file.c:97-116, 226-233): int16 I,Q interleaved for complex modes, int16
  * I only for real modes. With htv_set_sample_type the buffer holds that type
  * instead (the pointer keeps its int16_t type; size it in bytes). */

@@ -50,6 +50,12 @@ def main():
         run(mode, rate, 30, vfilter=filt, extra=tuple(extra) + ("--passthru",), source=f"passthru{ext_lines}",
             ext=T.passthru_stream(W, ext_lines))
         run(mode, rate, 30, vfilter=filt, extra=extra)
+    for mode, rate, nlines, filt, extra in T.POST_OFFSET:
+        run(mode, rate, nlines, vfilter=filt, extra=extra)
+    for mode, rate, filt, extra, ext_lines in T.POST_PASSTHRU:
+        W = orc.Oracle(T._conf(H, mode, filt, extra), rate).width
+        run(mode, rate, T.POST_LINES, vfilter=filt, extra=tuple(extra) + ("--passthru",), source=f"passthru{ext_lines}",
+            ext=T.passthru_stream(W, ext_lines))
 
     lines = {}
     for mode, rate in (("i", 16000000), ("pal", 16000000), ("l", 16000000), ("secam", 16000000), ("pal", 13500000)):

@@ -201,6 +201,51 @@ PASSTHRU_CASES = [
 ]
 
 
+def _post_stage_cases():
+    """Every row of the device's post-modulation matrix (test_gpu_zz_post_stage.py), without sound as it renders them:
+    (mode, rate, lines, vfilter, extra) of --offset f --swap-iq over its offset window on the complex rows, and (mode,
+    rate, vfilter, extra, external lines) of --passthru over its calls, the external stream cut off mid-line inside them."""
+    import test_gpu_zz_post_stage as P
+    offset, passthru = [], []
+    for i, (mode, rate, kw, W, _, _, cpx) in enumerate(P.ROWS):
+        filt = bool(kw.get("vfilter"))
+        quiet = ("--noaudio",) + (("--nocolour",) if kw.get("nocolour") else ())
+        if cpx:
+            offset.append((mode, rate, sum(P._offset_calls(W, kw)), filt,
+                           quiet + ("--offset", str(P._offset(rate, i)), "--swap-iq")))
+        passthru.append((mode, rate, filt, quiet, P._delay(kw) + P.PT_LINES))
+    return offset, passthru
+
+
+POST_OFFSET, POST_PASSTHRU = _post_stage_cases()
+POST_LINES = 114                            # sum(test_gpu_zz_post_stage.PT_CALLS)
+
+
+@pytest.mark.parametrize("mode,rate,nlines,filt,extra", POST_OFFSET)
+def test_offset_and_swap_at_the_post_stage_rows(built, mode, rate, nlines, filt, extra):
+    """The offset mixer's start-up window and the NCO after it, behind the IQ swap, at every complex row's width (in
+    HEAP_CASES with the reference's SECAM heap padding, ref_heap)"""
+    o = orc.Oracle(_conf(built, mode, filt, extra), rate, ref_heap=(mode, rate) in HEAP_CASES)
+    o.open_test_source()
+    got = o.render(nlines)
+    o.close()
+    assert_reference(got, ref_key(mode, rate, nlines, vfilter=filt, extra=extra))
+
+
+@pytest.mark.parametrize("mode,rate,filt,extra,ext_lines", POST_PASSTHRU)
+def test_passthru_at_the_post_stage_rows(built, mode, rate, filt, extra, ext_lines):
+    import test_gpu_zz_post_stage as P
+    assert sum(P.PT_CALLS) == POST_LINES
+    o = orc.Oracle(_conf(built, mode, filt, extra), rate, ref_heap=(mode, rate) in HEAP_CASES)
+    ext = passthru_stream(o.width, ext_lines)
+    o.open_test_source()
+    o.set_passthru(ext)
+    got = o.render(POST_LINES)
+    o.close()
+    assert_reference(got, ref_key(mode, rate, POST_LINES, vfilter=filt, extra=tuple(extra) + ("--passthru",),
+                                  source=f"passthru{ext_lines}"))
+
+
 @pytest.mark.parametrize("mode,rate,filt,extra,ext_lines", PASSTHRU_CASES)
 def test_passthru_alignment(built, mode, rate, filt, extra, ext_lines):
     """ref _vid_passthru_process video.c:3517-3541: line alignment (the external stream's first
