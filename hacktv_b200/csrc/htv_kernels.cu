@@ -89,6 +89,12 @@ struct DevTables {
 	int16_t *comp_q;                  // S-Video: the chroma term of each row (Q), same layout; NULL otherwise
 	int32_t comp_phases, comp_black;  // colour-frame phases; the black slot
 	int64_t comp_start;               // row of the first stream-start row
+	// filtered store of the k_line forms with a video filter and a composite store (k_vf_rows): each composite-store row
+	// of lines 2 .. lines - 1 after the video filter, as the line kernel holds it before the sound carriers - I | Q << 16,
+	// S-Video's chroma added to Q - at the composite row's index; NULL on every other path
+	uint32_t *filt;
+	uint32_t *vfx;                    // the call's filtered rows of the lines vf_exception lists, [list index][W]
+	int *vf_list;                     // [0]: how many; [1 + k]: raster descriptor entry of row k of vfx
 	// converted picture store of the k_line encoders whose subcarrier does not repeat within 4 frames (k_picture; k_line's
 	// PS forms): [slot][row][W], slot max_slots = black, row as htv_tables.c build_pic_rows; NULL on every other path
 	const int4 *pic_rows;             // [pic_nrows] line (1-based, 0 none), al, ar, keep of the line that shows the row
@@ -223,6 +229,7 @@ struct htv_dev_t {
 	cudaEvent_t ev_pic;               // upload stream, so that the next copies do not queue behind the conversions
 	cudaEvent_t *ev_slot;             // [max_slots] the copy of each slot's last picture is done
 	uint8_t *comp_valid;              // [max_slots] the phases of each slot's composite rows that hold its picture (bit p)
+	int *vf_conv, vf_nconv;           // filtered store: the composite-store entries converted since the last k_vf_rows
 	int pic_pending;                  // conversions were launched that the caller's stream has not waited for yet
 	unsigned chunk_i;
 	cudaEvent_t ev_in, ev_audio;
@@ -236,6 +243,9 @@ struct htv_dev_t {
 	void *d_desc_r;                   // raster descriptors [cap + before + after] (x 2 for the fused line kernel): LineS2 for
 	                                  // SECAM, LineR2 for PAL / NTSC / mono
 	void *d_desc_a2;                  // LineA2[cap + 1] (x 2 for the fused line kernel)
+	uint32_t *d_vfx;                  // filtered store: the call's rows of the lines vf_exception lists, [vf_cap][W] x 2 ...
+	int *d_vfl;                       // ... and their list, [1 + vf_cap] x 2, beside the raster descriptors
+	int vf_cap;
 	int desc_cap;                     // lines per call the descriptor buffers hold (desc_reserve)
 	int kl_ctas;                      // persistent CTAs of the fused kernels (k_line, k_sec_raster)
 	char kname[192];                  // the line kernel(s) the last render launched, with their template arguments (htv_line_kernel)
@@ -748,8 +758,44 @@ __device__ __forceinline__ bool line_overlay(const DevTables &dt, int64_t L, int
 	return(true);
 }
 
+// the row of the composite store scan line L shows: of its frame's picture at its colour-frame phase, of the black slot
+// where the frame has none; the stream-start rows for L <= 0
+__device__ __forceinline__ long long comp_row(const htv_dparams_t &dp, const DevTables &dt, int64_t L)
+{
+	if(L <= 0) return(dt.comp_start + (L < 0 ? 0 : 1));
+	const int64_t f0 = L / dp.lines;
+	const int slot = frame_slot(dt, f0);
+	return(((long long) (slot >= 0 ? slot : dt.comp_black) * dt.comp_phases + f0 % dt.comp_phases) * dp.lines + (L - f0 * dp.lines));
+}
+
+// The lines whose filtered row is not the filtered store's: the video filter of line L reads lines L - 1 .. L + 1
+// (32-sample halos on the neighbours), which are rows of one (slot, phase) entry of the composite store, without
+// overlays, unless L is the first or last line of its frame, reaches the stream-start rows (L <= 1), or an overlay line
+// is among them. The one place that decides it (k_line_desc_r lists them, k_vf_rows filters the list).
+__device__ __forceinline__ bool vf_exception(const htv_dparams_t &dp, const DevTables &dt, int64_t L)
+{
+	if(L <= 1) return(true);
+	const int line = (int) (L % dp.lines);                        // 0-based
+	if(line == 0 || line == dp.lines - 1) return(true);
+	if(dt.ov_n <= 0) return(false);
+	int lo = 0, hi = dt.ov_n;                                       // the first overlay line >= L - 1 (dt.ov_line is sorted)
+	while(lo < hi) { const int mid = (lo + hi) >> 1; if(dt.ov_line[mid] < L - 1) lo = mid + 1; else hi = mid; }
+	return(lo < dt.ov_n && dt.ov_line[lo] <= L + 1);
+}
+
+// The most lines of a call with `rows` raster descriptors from line line0 - before (line0 >= 0) that vf_exception can
+// list: L <= 1 (before + 2 of them at most), the first and last line of every frame the rows touch, and each overlay line
+// with its two neighbours
+static int vf_list_bound(int rows, int before, int lines, int ov_n)
+{
+	const int n = before + 2 + 2 * (rows / lines + 2) + 3 * ov_n;
+	return(n < rows ? n : rows);
+}
+
 // Raster descriptors of lines first .. first + n - 1, entry i <-> line first + i, one thread per line: LineS2 rows for
-// SECAM, LineR2 rows for every other colour system
+// SECAM, LineR2 rows for every other colour system. With a filtered store (dt.filt), pic is the line's filtered row,
+// in the filtered store or, for the lines vf_exception lists (dt.vf_list, in no particular order), -1 - its index in
+// the list, which is its row of dt.vfx.
 __global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const DevTables dt, void *out, int64_t first, int n)
 {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -795,15 +841,12 @@ __global__ void k_line_desc_r(const __grid_constant__ htv_dparams_t dp, const De
 		const int slot = row < dp.active_lines ? frame_slot(dt, frame - 1) : -1;
 		o.pic = ((long long) (slot >= 0 ? slot : dt.pic_black) * dt.pic_nrows + row) * dp.W;
 	}
-	if(dt.comp)
+	if(dt.comp) o.pic = comp_row(dp, dt, L) * dp.W;
+	if(dt.filt && vf_exception(dp, dt, L))
 	{
-		long long row = dt.comp_start + (L < 0 ? 0 : 1);
-		if(L > 0)
-		{
-			const int slot = frame_slot(dt, frame - 1);
-			row = ((long long) (slot >= 0 ? slot : dt.comp_black) * dt.comp_phases + (frame - 1) % dt.comp_phases) * dp.lines + line - 1;
-		}
-		o.pic = row * dp.W;
+		const int k = atomicAdd(dt.vf_list, 1);
+		dt.vf_list[1 + k] = i;
+		o.pic = -1 - k;
 	}
 	reinterpret_cast<LineR2 *>(out)[i] = o;
 }
@@ -2705,7 +2748,9 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	if(p->kl)
 	{
 		kl_name(kl, sizeof(kl), *p->kl, type, dp.s_video);
-		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (vf ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
+		// the composite ring and the tap operand where k_line filters: the PS and SRC forms (htv_line.cuh)
+		const bool ring = vf && (p->kl->ps || p->kl->src);
+		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (ring ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
 		// PS forms with S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
 		if(dp.s_video && p->kl->ps) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
 	}
@@ -2748,6 +2793,17 @@ extern "C" int htv_dev_plan_name(const struct htv_tables_t *t, int sample_type, 
 	if(plan_kernels(t, dev_switches(), sample_type, &p, name, len) != HTV_OK) return(HTV_ERROR);
 	snprintf(name, len, "%s", p.kname);
 	return(HTV_OK);
+}
+
+// k_vf_rows over the store rows of the composite-store entries cv.e and, after them, nexc CTAs for the lines
+// k_line_desc_r listed (vf_exception) among the raster descriptors from line `first`
+static void launch_vf_rows(htv_dev_t *d, const VfConv &cv, int64_t first, int nexc, cudaStream_t st)
+{
+	const htv_dparams_t &dp = d->dp;
+	const unsigned grid = (unsigned) (cv.n * (dp.lines - 2) + nexc);
+	const size_t smem = 2 * ((size_t) mf_row_bytes(dp.W) + 16);
+	if(dp.vf_type == 3) k_vf_rows<true><<<grid, d->plan.kl_threads, smem, st>>>(dp, d->dt, cv, first);
+	else k_vf_rows<false><<<grid, d->plan.kl_threads, smem, st>>>(dp, d->dt, cv, first);
 }
 
 // An encoder's side streams and events, in the one list htv_dev_create creates and htv_dev_destroy destroys. ev0 and
@@ -2875,6 +2931,17 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		if(!d->comp_valid) return(create_fail(d, err, errlen, "out of memory"));
 		dt.comp = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
 		if(dp.s_video) dt.comp_q = (int16_t *) dev_zero(d, sizeof(int16_t) * n);
+		if(p.kl->vf)
+		{
+			// the filtered store (k_vf_rows): a row for every composite-store row but the stream-start rows, 4 bytes a
+			// sample (174 MB for PAL at 16 Msps). One k_vf_rows launch per call takes every pending conversion.
+			if(d->max_slots * dt.comp_phases > VF_CONV)
+				return(create_fail(d, err, errlen, "%d picture slots x %d phases: more conversions than k_vf_rows takes (%d)",
+					d->max_slots, dt.comp_phases, VF_CONV));
+			d->vf_conv = (int *) calloc((size_t) d->max_slots * dt.comp_phases, sizeof(int));
+			if(!d->vf_conv) return(create_fail(d, err, errlen, "out of memory"));
+			dt.filt = (uint32_t *) dev_zero(d, sizeof(uint32_t) * (size_t) dt.comp_start * dp.W);
+		}
 	}
 	dt.pcm = d->d_pcm;
 	if(dp.have_fm)
@@ -3002,6 +3069,13 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 	{
 		for(int ph = 0; ph < t->comp_phases; ph++) k_compose<<<dp.lines, p.line_threads, p.raster_smem>>>(dp, dt, dt.comp_black, ph, 0);
 		k_compose<<<2, p.line_threads, p.raster_smem>>>(dp, dt, dt.comp_black, 0, 1);
+		if(dt.filt)
+		{
+			VfConv cv;
+			cv.n = t->comp_phases;
+			for(int ph = 0; ph < cv.n; ph++) cv.e[ph] = dt.comp_black * cv.n + ph;
+			launch_vf_rows(d, cv, 0, 0, 0);
+		}
 	}
 	const DevSync sy = dev_sync(d);
 	bool made = true;
@@ -3024,7 +3098,7 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	// the side streams may still be ahead of the caller's; nothing of this encoder is freed under running work
 	cudaDeviceSynchronize();
 	for(int i = 0; i < d->nalloc; i++) cudaFree(d->alloc[i]);
-	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_comp); cudaFree(d->d_compq); cudaFree(d->d_comp32); cudaFree(d->d_planes);
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_vfx); cudaFree(d->d_vfl); cudaFree(d->d_comp); cudaFree(d->d_compq); cudaFree(d->d_comp32); cudaFree(d->d_planes);
 	if(d->h_map) cudaFreeHost(d->h_map);
 	if(d->h_ov_line) { cudaFreeHost(d->h_ov_line); cudaFreeHost(d->h_ov_meta); cudaFreeHost(d->h_ov_add); }
 	cudaFree(d->d_ov_line); cudaFree(d->d_ov_meta); cudaFree(d->d_ov_add);
@@ -3035,6 +3109,7 @@ extern "C" void htv_dev_destroy(htv_dev_t *d)
 	for(cudaEvent_t *e : sy.timed) if(*e) cudaEventDestroy(*e);
 	for(cudaEvent_t *e : sy.event) if(*e) cudaEventDestroy(*e);
 	free(d->comp_valid);
+	free(d->vf_conv);
 	if(d->ev_slot) for(int i = 0; i < d->max_slots; i++) if(d->ev_slot[i]) cudaEventDestroy(d->ev_slot[i]);
 	free(d->ev_slot);
 	free(d);
@@ -3165,6 +3240,12 @@ static int convert_frames(htv_dev_t *d, const int32_t *slot_of_frame, int n, int
 		d->launches++;
 		CK(cudaGetLastError());
 		d->comp_valid[s] |= (uint8_t) (1u << ph);
+		if(d->dt.filt)
+		{
+			int k = 0;
+			while(k < d->vf_nconv && d->vf_conv[k] != s * P + ph) k++;
+			if(k == d->vf_nconv) d->vf_conv[d->vf_nconv++] = s * P + ph;
+		}
 		d->pic_pending = 1;
 	}
 	if(d->pic_pending)
@@ -3322,13 +3403,20 @@ static int desc_reserve(htv_dev_t *d, int n, cudaStream_t st)
 	cudaStreamSynchronize(d->side);
 	cudaStreamSynchronize(d->side2);
 	cudaStreamSynchronize(d->side3);
-	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2);
+	cudaFree(d->d_desc_r); cudaFree(d->d_desc_a2); cudaFree(d->d_vfx); cudaFree(d->d_vfl);
 	d->d_desc_r = d->d_desc_a2 = NULL;
+	d->d_vfx = NULL; d->d_vfl = NULL;
 	d->desc_cap = 0;
 	static_assert(sizeof(LineS2) == sizeof(LineR2), "one raster descriptor buffer holds either");
 	if(p.path != PATH_RS) CK(cudaMalloc(&d->d_desc_r, bufs * sizeof(LineR2) * ((size_t) n + p.before + p.after)));
 	// + 1: FM video's fill line (fm_skip)
 	if(p.path != PATH_RASTER) CK(cudaMalloc(&d->d_desc_a2, bufs * sizeof(LineA2) * ((size_t) n + 1)));
+	if(d->dt.filt)
+	{
+		d->vf_cap = vf_list_bound(n + p.before + p.after, p.before, d->dp.lines, HTV_OV_CAP);
+		CK(cudaMalloc(&d->d_vfx, bufs * sizeof(uint32_t) * d->vf_cap * d->dp.W));
+		CK(cudaMalloc(&d->d_vfl, bufs * sizeof(int) * (1 + d->vf_cap)));
+	}
 	d->desc_cap = n;
 	return(HTV_OK);
 }
@@ -3342,8 +3430,29 @@ static int launch_desc_r(htv_dev_t *d, htv_dev_t *c, int64_t line0, int n, cudaS
 	const int rows = n + p.before + p.after;
 	const bool side = c->ahead && c->r2_armed;
 	*lr = (char *) c->d_desc_r + (size_t) c->kl_buf * sizeof(LineR2) * ((size_t) c->desc_cap + p.before + p.after);
-	k_line_desc_r<<<(rows + 63) / 64, 64, 0, side ? c->side3 : st>>>(c->dp, c->dt, *lr, line0 - p.before, rows);
+	const cudaStream_t s = side ? c->side3 : st;
+	if(c->dt.filt)
+	{
+		// the lines of this call that vf_exception lists, and their filtered rows, in the descriptor buffers' half
+		c->dt.vf_list = c->d_vfl + (size_t) c->kl_buf * (1 + c->vf_cap);
+		c->dt.vfx = c->d_vfx + (size_t) c->kl_buf * c->vf_cap * c->dp.W;
+		CK(cudaMemsetAsync(c->dt.vf_list, 0, sizeof(int), s));
+	}
+	k_line_desc_r<<<(rows + 63) / 64, 64, 0, s>>>(c->dp, c->dt, *lr, line0 - p.before, rows);
 	d->launches++;
+	if(c->dt.filt)
+	{
+		// the video filter of those lines and of the store rows of this call's conversions, in one launch per call (the
+		// pending conversions are distinct entries, at most max_slots x comp_phases <= VF_CONV: htv_dev_create). The
+		// conversions ran on the pic stream: the caller's stream has waited for them (convert_frames), side3 waits here
+		if(side && c->vf_nconv) CK(cudaStreamWaitEvent(s, c->ev_pic, 0));
+		VfConv cv;
+		cv.n = c->vf_nconv;
+		for(int k = 0; k < cv.n; k++) cv.e[k] = c->vf_conv[k];
+		launch_vf_rows(c, cv, line0 - p.before, vf_list_bound(rows, p.before, c->dp.lines, c->dt.ov_n), s);
+		d->launches++;
+		c->vf_nconv = 0;
+	}
 	if(side)
 	{
 		CK(cudaEventRecord(c->ev_r2, c->side3));

@@ -38,6 +38,37 @@ __device__ __forceinline__ int kl_acc15(int hh, int mid, int ll)
 }
 __device__ __forceinline__ int kl_fir_out(int hh, int mid, int ll) { return(sat16i(kl_acc15(hh, mid, ll))); }
 
+// The 51-tap VSB / low-pass video filter on the tensor cores, one tile of 128 samples per warp: ph is the lane's first
+// byte (mf_b_offset) of the staged row's high-byte plane, the low-byte plane RB bytes on; atab the tap operand
+// ([k-step][I hi, I lo, Q hi, Q lo][lane], shared or global memory). The lane's outputs at xb + 8 j go to oi / oq.
+template<bool HASQ>
+__device__ __forceinline__ void kl_vfilter(const unsigned char *ph, int RB, const uint4 *atab, int lane, int (&oi)[4], int (&oq)[4])
+{
+	const unsigned char *plo = ph + RB;
+	int ihh[4] = { 0, 0, 0, 0 }, imid[4] = { 0, 0, 0, 0 }, ill[4] = { 0, 0, 0, 0 };
+	int qhh[4] = { 0, 0, 0, 0 }, qmid[4] = { 0, 0, 0, 0 }, qll[4] = { 0, 0, 0, 0 };
+	#pragma unroll
+	for(int s = 0; s < MF_KSTEPS; s++)
+	{
+		const uint2 xh = *reinterpret_cast<const uint2 *>(ph + 32 * s);
+		const uint2 xl = *reinterpret_cast<const uint2 *>(plo + 32 * s);
+		const uint4 aih = atab[(s * 4 + 0) * 32 + lane], ail = atab[(s * 4 + 1) * 32 + lane];
+		mma_ss(ihh, aih, xh); mma_su(imid, aih, xl); mma_us(imid, ail, xh); mma_uu(ill, ail, xl);
+		if(HASQ)
+		{
+			const uint4 aqh = atab[(s * 4 + 2) * 32 + lane], aql = atab[(s * 4 + 3) * 32 + lane];
+			mma_ss(qhh, aqh, xh); mma_su(qmid, aqh, xl); mma_us(qmid, aql, xh); mma_uu(qll, aql, xl);
+		}
+	}
+	#pragma unroll
+	for(int j = 0; j < 4; j++)
+	{
+		const int ci = mf_lane_ci(j);
+		oi[j] = kl_fir_out(ihh[ci], imid[ci], ill[ci]);
+		oq[j] = HASQ ? kl_fir_out(qhh[ci], qmid[ci], qll[ci]) : 0;
+	}
+}
+
 // Mixers after the modulation (htv_sound.cuh), channel combiner, store in the strided layout.
 // ST: the sample type the store converts to (htv_sample_type.h), -1 for dp.sample_type at run time. The channel combiner
 // (`acc`, int16 in the output layout) still adds in int16 with wrap-around; the conversion is the last step, as the
@@ -98,11 +129,16 @@ __device__ __forceinline__ void kl_cp16(void *dst_smem, const void *src)
 }
 __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// VF: a video filter is on (composite ring + tensor-core FIR); HASQ: it has Q taps (VSB); FULL: 128 | W (no
+// VF: a video filter is on; HASQ: it has Q taps (VSB); FULL: 128 | W (no
 // partial tile: the x < W tests fold away); CSAT: the chroma low-pass can leave the int16 range (sum of |taps| > 32768),
 // which k_compose's saturating low-pass handles when it fills the store: the CSAT forms run the same code as the others
 //
-// Per iteration q (one scan line) a CTA runs
+// The forms with a video filter and a composite store (FS: VF, not PS, not SRC) do not filter: k_vf_rows filtered each
+// line's three composite rows and overlays once, into the filtered store (a row per line of each slot and phase) or,
+// for the lines whose filter window leaves one frame's rows or meets an overlay, into the call's own rows. Per
+// iteration q they load line q + 1's filtered I | Q (R1), and give line q its sound carriers and store it (M).
+//
+// Every other form, per iteration q (one scan line), runs
 //   R2(q)   VBI overlay on the values fetched earlier, composite row q mod 4                  | __syncthreads
 //   R1(q+1) the composite row of the NEXT line is loaded here ...
 //   M(q-1)  ... and arrive while line q - 1 (whose right-hand halo R2(q) has just written) is filtered (mma),
@@ -123,7 +159,8 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 //
 // S-Video (KL_SV, dp.s_video; ref video.c:3031-3040, 3206-3228): the subcarrier term goes to Q instead of I, and the
 // video filter runs on I only, so Q of the stored line is that line's own chroma. k_compose wrote it into the store's
-// chroma plane (dt.comp_q), which M reads at the row of mrow; SRC: the chain wrote Q into its own plane, `srcq`; PS: R2
+// chroma plane (dt.comp_q), which M reads at the row of mrow (FS: k_vf_rows added it to Q of the filtered row); SRC: the
+// chain wrote Q into its own plane, `srcq`; PS: R2
 // parks it in a two-row ring in shared memory at the lane's own slots (row q & 1), which M takes back for mrow.
 template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16,
 	bool PS = false>
@@ -132,14 +169,16 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr, const int16_t *srcq = nullptr)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
+	// FS: the filtered store holds each line's filter output (k_vf_rows); RING: the filter runs here, on the ring
+	constexpr bool FS = VF && !PS && !SRC, RING = VF && !FS;
 	const int W = WC ? WC : dp.W;
 	const int RB = kl_row_bytes(W);
-	// descriptors x2 | [row 0..3][hi, lo] composite planes | FIR taps | NICAM pulse | PS, S-Video: chroma [row 0..1][j][thread]
+	// descriptors x2 | RING: [row 0..3][hi, lo] composite planes, FIR taps | NICAM pulse | PS, S-Video: chroma [row 0..1][j][thread]
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
 	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + 2);
 	unsigned char *rows = reinterpret_cast<unsigned char *>(slr + 2);
-	uint4 *atab = reinterpret_cast<uint4 *>(rows + (VF ? 8 * RB : 0));    // [k-step][I hi, I lo, Q hi, Q lo][lane]
-	short *ntp = reinterpret_cast<short *>(atab + (VF ? MF_ATAB_WORDS / 4 : 0));
+	uint4 *atab = reinterpret_cast<uint4 *>(rows + (RING ? 8 * RB : 0));  // [k-step][I hi, I lo, Q hi, Q lo][lane]
+	short *ntp = reinterpret_cast<short *>(atab + (RING ? MF_ATAB_WORDS / 4 : 0));
 	const int tid = threadIdx.x, lane = tid & 31, nt = tid >> 5;
 	const int g = lane >> 2, t = lane & 3;
 	const int xb = mf_lane_x(nt, lane, 0);                                  // the lane's samples: xb + 8 j
@@ -149,11 +188,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	const int a = blockIdx.x * run, bnd = min(a + run, nlines);
 	if(a >= nlines) return;
 	// relative line q: raster lines a-1 .. bnd (descriptor lrp[q + 1]), modulate a .. bnd-1
-	const int q0 = VF ? a - 1 : a, q1 = VF ? bnd : bnd - 1;
+	const int q0 = RING ? a - 1 : a, q1 = RING ? bnd : bnd - 1;
 
 	// ---- one-time set-up -------------------------------------------------------
-	if(VF) for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
-	if(VF) for(int i = tid; i < 8 * RB / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
+	if(RING) for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
+	if(RING) for(int i = tid; i < 8 * RB / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
 	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
 	{
 		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
@@ -169,11 +208,19 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	const int fo0 = mf_b_offset(nt, 0, lane);
 	constexpr int NA16 = (int) (sizeof(LineA2) / 16);
 
-	// loads of line q issued one phase early: the line's composite row (int16 x 4); PS: line values (int16 x 4) and, on
-	// colour lines, filtered U | V << 16 (x 4)
+	// loads of line q issued one phase early: the line's composite row (int16 x 4); FS: the line's filtered I | Q << 16
+	// (x 4), from the filtered store or, for the lines k_line_desc_r listed (pic < 0), from the call's rows at the list
+	// index; PS: line values (int16 x 4) and, on colour lines, filtered U | V << 16 (x 4)
 	int tm[4];
 	unsigned px[4];
 	#define KL_R1(QQ) do { \
+		if(FS) \
+		{ \
+			const long long pic_ = slr[(QQ) & 1].pic; \
+			const uint32_t *fp_ = (pic_ >= 0 ? dt.filt + pic_ : dt.vfx + (size_t) (-1 - pic_) * W) + xb; \
+			_Pragma("unroll") for(int j = 0; j < 4; j++) px[j] = (FULL || xb + 8 * j < W) ? __ldg(fp_ + 8 * j) : 0u; \
+			break; \
+		} \
 		if(!PS) \
 		{ \
 			const int16_t *tp_ = SRC ? src + (size_t) ((QQ) + 2) * W + xb : dt.comp + slr[(QQ) & 1].pic + xb; \
@@ -192,12 +239,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		else { px[0] = px[1] = px[2] = px[3] = 0u; } \
 	} while(0)
 	KL_R1(q0);
-	int ppic = 0;                                                           // S-Video: the row of line q - 1 (< 2^31, htv_dev_create)
 
 	int r4 = q0 & 3;                                                        // ring row of line q
 	for(int q = q0; q <= q1; q++, r4 = (r4 + 1) & 3)
 	{
-		const int mrow = VF ? q - 1 : q;                                    // the line modulated in this iteration
+		const int mrow = RING ? q - 1 : q;                                  // the line modulated in this iteration
 		// ---- descriptors of the next raster line and of the line modulated below -> shared memory -----
 		if(tid < 4) { if(!SRC && q + 1 <= q1) kl_cp16(reinterpret_cast<int4 *>(slr + ((q + 1) & 1)) + tid, reinterpret_cast<const int4 *>(lrp + q + 2) + tid); }
 		else if(tid < 4 + NA16) { if(mrow >= a) kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + (tid - 4), reinterpret_cast<const int4 *>(lap + mrow) + (tid - 4)); }
@@ -210,8 +256,8 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		// ---- R2: (PS: burst, subcarrier,) VBI overlay of line q ---------------------
 		const LineR2 &li = slr[q & 1];
 		int val[4] = { tm[0], tm[1], tm[2], tm[3] };
-		int mpic = 0;                                                       // S-Video: the row of the line modulated below
-		if(!SRC && !PS && sv) { mpic = VF ? ppic : (int) li.pic; ppic = (int) li.pic; }
+		const unsigned fv[4] = { px[0], px[1], px[2], px[3] };              // FS: the filtered line q
+		const int mpic = !VF && !SRC && !PS && sv ? (int) li.pic : 0;       // S-Video: the row of the line (< 2^31, htv_dev_create)
 		int cq[4] = { 0, 0, 0, 0 };                                         // PS, S-Video: the chroma of line q
 		if(PS && li.pal)
 		{
@@ -255,7 +301,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 			#pragma unroll
 			for(int j = 0; j < 4; j++) svq[((q & 1) * 4 + j) * blockDim.x + tid] = (short) cq[j];
 		}
-		if(!SRC && li.ov_any)
+		if(!SRC && !FS && li.ov_any)
 		{
 			// VBI stages run on the finished line (ref video.c:4213-4357 register them behind the raster)
 			#pragma unroll
@@ -268,7 +314,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		}
 
 		const int rprev = r4 == 0 ? 3 : r4 - 1, rnext = r4 == 3 ? 0 : r4 + 1;   // ring rows of lines q - 1, q + 1
-		if(VF)
+		if(RING)
 		{
 			// ---- composite line -> ring row q mod 4 (+ the neighbours' halos) ----------
 			unsigned char *rp = rows + (2 * r4) * RB + KL_LEAD + xb;
@@ -307,32 +353,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		if(mrow < a) continue;
 
 		int oi[4], oq[4];
-		if(VF)
+		if(RING) kl_vfilter<HASQ>(rows + (2 * rprev) * RB + fo0, RB, atab, lane, oi, oq);   // ---- M: video filter of line q - 1
+		else if(FS)
 		{
-			// ---- M: video filter of line q - 1, one tile of 128 samples per warp -------
-			const unsigned char *ph = rows + (2 * rprev) * RB + fo0, *plo = ph + RB;
-			int ihh[4] = { 0, 0, 0, 0 }, imid[4] = { 0, 0, 0, 0 }, ill[4] = { 0, 0, 0, 0 };
-			int qhh[4] = { 0, 0, 0, 0 }, qmid[4] = { 0, 0, 0, 0 }, qll[4] = { 0, 0, 0, 0 };
 			#pragma unroll
-			for(int s = 0; s < MF_KSTEPS; s++)
-			{
-				const uint2 xh = *reinterpret_cast<const uint2 *>(ph + 32 * s);
-				const uint2 xl = *reinterpret_cast<const uint2 *>(plo + 32 * s);
-				const uint4 aih = atab[(s * 4 + 0) * 32 + lane], ail = atab[(s * 4 + 1) * 32 + lane];
-				mma_ss(ihh, aih, xh); mma_su(imid, aih, xl); mma_us(imid, ail, xh); mma_uu(ill, ail, xl);
-				if(HASQ)
-				{
-					const uint4 aqh = atab[(s * 4 + 2) * 32 + lane], aql = atab[(s * 4 + 3) * 32 + lane];
-					mma_ss(qhh, aqh, xh); mma_su(qmid, aqh, xl); mma_us(qmid, aql, xh); mma_uu(qll, aql, xl);
-				}
-			}
-			#pragma unroll
-			for(int j = 0; j < 4; j++)
-			{
-				const int ci = mf_lane_ci(j);
-				oi[j] = kl_fir_out(ihh[ci], imid[ci], ill[ci]);
-				oq[j] = HASQ ? kl_fir_out(qhh[ci], qmid[ci], qll[ci]) : 0;
-			}
+			for(int j = 0; j < 4; j++) { oi[j] = (int) (short) (fv[j] & 0xFFFFu); oq[j] = (int) fv[j] >> 16; }
 		}
 		else
 		{
@@ -343,9 +368,9 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		// ---- sound carriers, mixers, store ---------------------------------------
 		if(FULL || xb < W)
 		{
-			if(sv)
+			if(sv && !FS)
 			{
-				// Q = the chroma of line mrow (the video filter leaves it alone)
+				// Q = the chroma of line mrow (the video filter leaves it alone; FS: k_vf_rows added it)
 				const int16_t *qp = (SRC ? srcq + (size_t) (mrow + 2) * W : PS ? srcq : dt.comp_q + mpic) + xb;
 				#pragma unroll
 				for(int j = 0; j < 4; j++)
@@ -360,4 +385,82 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		}
 	}
 	#undef KL_R1
+}
+
+// ---------------------------------------------------------------------------
+// k_vf_rows: the video filter of the k_line forms with a composite store (FS), once per row instead of once per line of
+// every frame. A CTA filters one line, a warp one tile of 128 samples, as k_line's M stage did: the three composite rows
+// of lines L - 1 .. L + 1 (32-sample halos on the neighbours) go into a row of byte planes in shared memory exactly as
+// k_line's ring held them, with their VBI overlays; the output is the pair k_line holds before the sound carriers,
+// I | Q << 16, with S-Video's chroma added to Q.
+//   blocks [0, cv.n (lines - 2)): the filtered store's rows of lines 2 .. lines - 1 of the composite-store entries cv.e
+//            (slot * comp_phases + phase) - rows of one entry, no overlays
+//   the rest: row k of dt.vfx, line first + dt.vf_list[1 + k], for k < dt.vf_list[0] (vf_exception)
+// ---------------------------------------------------------------------------
+#define VF_CONV 64                    // composite-store entries one launch filters: all of a call's (htv_dev_create checks)
+struct VfConv { int n; int e[VF_CONV]; };
+
+template<bool HASQ>
+__global__ void __launch_bounds__(384)
+k_vf_rows(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const __grid_constant__ VfConv cv, int64_t first)
+{
+	extern __shared__ __align__(16) unsigned char smem_raw[];
+	__shared__ int4 som[3];                                             // the overlays of lines L - 1 .. L + 1
+	__shared__ int sov[3];
+	const int W = dp.W, RB = kl_row_bytes(W), N = dp.lines;
+	const int tid = threadIdx.x, lane = tid & 31;
+	const int ns = cv.n * (N - 2);
+	long long row[3];                                                   // composite rows of lines L - 1, L, L + 1
+	uint32_t *dst;
+	const bool exc = (int) blockIdx.x >= ns;
+	if(!exc)
+	{
+		const long long r = (long long) cv.e[blockIdx.x / (N - 2)] * N + blockIdx.x % (N - 2) + 1;
+		row[0] = r - 1; row[1] = r; row[2] = r + 1;
+		dst = dt.filt + r * W;
+	}
+	else
+	{
+		const int k = blockIdx.x - ns;
+		if(k >= dt.vf_list[0]) return;
+		const int64_t L = first + dt.vf_list[1 + k];
+		#pragma unroll
+		for(int d = 0; d < 3; d++) row[d] = comp_row(dp, dt, L - 1 + d);
+		dst = dt.vfx + (size_t) k * W;
+		if(tid < 3) sov[tid] = line_overlay(dt, L - 1 + tid, som[tid]);
+		__syncthreads();
+	}
+
+	// ---- the composite window of line L -> [hi, lo] byte planes (byte b = sample b - KL_LEAD) --------------
+	unsigned char *ph = smem_raw;
+	for(int b = tid; b < RB; b += blockDim.x)
+	{
+		const int x = b - KL_LEAD, d = x < 0 ? 0 : x < W ? 1 : 2, xs = x - (d - 1) * W;
+		int val = 0;
+		if(d != 2 || x < W + KL_LEAD)
+		{
+			val = dt.comp[row[d] * W + xs];
+			if(exc && sov[d])
+			{
+				const int4 m = som[d];
+				if(xs >= m.x && xs < m.y) val = m.z;
+				if(m.w >= 0) val = wrap16i(val) + dt.ov_add[(size_t) m.w * W + xs];
+			}
+		}
+		ph[b] = (unsigned char) (val >> 8);
+		ph[RB + b] = (unsigned char) val;
+	}
+	__syncthreads();
+
+	int oi[4], oq[4];
+	const int nt = tid >> 5, xb = mf_lane_x(nt, lane, 0);
+	kl_vfilter<HASQ>(ph + mf_b_offset(nt, 0, lane), RB, reinterpret_cast<const uint4 *>(dt.mma_atab), lane, oi, oq);
+	#pragma unroll
+	for(int j = 0; j < 4; j++)
+	{
+		const int x = xb + 8 * j;
+		if(x >= W) continue;
+		if(dp.s_video) oq[j] += dt.comp_q[row[1] * W + x];
+		dst[x] = ((unsigned) oi[j] & 0xFFFFu) | ((unsigned) oq[j] << 16);
+	}
 }
