@@ -87,6 +87,12 @@ typedef struct {
 	int32_t swap_iq, have_offset;
 	uint64_t offset_ang;           /* turns * 2^64 per sample */
 	uint64_t offset_phase0;        /* phase after the first renormalisation (see htv_tables.c) */
+
+	/* k_line's sound feed (htv_line.cuh KlFeed): what one line of W samples adds to each quotient and remainder of a
+	 * lane's state; set by htv_dev_create where k_line modulates */
+	int32_t kl_w_kk, kl_w_cc;      /* W mod 32767, W mod nicam_cc_len */
+	uint32_t kl_w_aq, kl_w_ar;     /* 32000 W = kl_w_aq rate + kl_w_ar */
+	uint32_t kl_w_sq, kl_w_sr;     /* W nicam_D = kl_w_sq nicam_F + kl_w_sr */
 } htv_dparams_t;
 
 #ifdef __CUDACC__

@@ -53,6 +53,15 @@ struct DevGuard {
 	~DevGuard() { if(switched) cudaSetDevice(prev); }
 };
 
+// The record of audio index j for k_line's sound feed (htv_line.cuh), slot (j + 1) & (RA - 1): B(j), the phase
+// accumulated before j's segment starts (for j = -1 one angle step less: see kl_lane_feed), the angle step of j's
+// modulating sample and (cos, sin) of 8 of those steps (k_fm_scan_fix)
+struct __align__(16) SegRec {
+	ulonglong2 ba;                    // B(j), step
+	float2 rot;
+	float pad[2];
+};
+
 struct DevTables {
 	const uint32_t *mma_atab;         // tap operand of the tensor-core video filter, fragment order (htv_mma_fir.h)
 	const int16_t *tmpl_out, *tmpl_keep;   // line templates: blank + sync pulses (htv_tables.c build_templates)
@@ -112,6 +121,10 @@ struct DevTables {
 	uint8_t *nic_local;               // RS: inclusive prefix (mod 4) of the DQPSK steps inside the symbol's frame
 	uint8_t *nic_ftot;                // RF: total step of frame k (mod 4)
 	uint8_t *nic_fstart;              // RF: differential symbol state before frame k
+	// records of k_line's sound feed (htv_line.cuh), written behind the pre-pass chains; NULL on the other paths
+	SegRec *seg_rec;                  // RA, slot (j + 1) & (RA - 1): audio index j
+	uint32_t *nic_rec;                // RS, slot s & (RS - 1): NICAM symbol s - pulse-table rows of its 6-symbol pattern,
+	                                  // I (bits 0-8) and Q (9-17); its DQPSK polarities (18-19: symc's code); bit 20: no row
 	// VBI overlays of the current launch sequence (sorted by global line index)
 	int ov_n;
 	const long long *ov_line;         // [ov_n] global line index
@@ -217,6 +230,7 @@ struct htv_dev_t {
 	// carries
 	int64_t fm_jc;                    // last audio index whose fm_B entry is valid (-1 at start)
 	int64_t nic_kc;                   // first frame whose nic_fstart is valid for a restart
+	int64_t fm_jr, nic_kr;            // last audio index / NICAM frame with records (dt.seg_rec, dt.nic_rec)
 	uint64_t launches;
 	int timing;
 	cudaEvent_t ev0, ev1;
@@ -423,7 +437,8 @@ __global__ void __launch_bounds__(SCAN_T) k_fm_scan_local(const DevTables dt, in
 	if(t == SCAN_T - 1) dt.scan_tot[blockIdx.x] = part[t];
 }
 
-__global__ void __launch_bounds__(SCAN_T) k_fm_scan_fix(const DevTables dt, int64_t jc, int64_t j1)
+// Also the records of k_line's sound feed (dt.seg_rec) for the audio indices past jr, whose B(j) is final here
+__global__ void __launch_bounds__(SCAN_T) k_fm_scan_fix(const DevTables dt, int64_t jc, int64_t j1, int64_t jr)
 {
 	__shared__ unsigned long long off;
 	const int t = threadIdx.x;
@@ -440,7 +455,19 @@ __global__ void __launch_bounds__(SCAN_T) k_fm_scan_fix(const DevTables dt, int6
 	for(int i = 0; i < SCAN_PER; i++)
 	{
 		const int64_t j = a + i;
-		if(j <= j1) dt.fm_B[(j + 1) & (RA - 1)] += off;
+		if(j > j1) continue;
+		const unsigned long long B = dt.fm_B[(j + 1) & (RA - 1)] + off;
+		dt.fm_B[(j + 1) & (RA - 1)] = B;
+		if(dt.seg_rec && j > jr)
+		{
+			const int pi = (int) dt.fm_p[(j + 1) & (RA - 1)] + 32768;
+			const unsigned long long ang = dt.fm_ang[pi];
+			SegRec r;
+			r.ba = make_ulonglong2(j < 0 ? B - ang : B, ang);
+			r.rot = dt.fm_rot8[pi];
+			r.pad[0] = r.pad[1] = 0.0f;
+			dt.seg_rec[(j + 1) & (RA - 1)] = r;
+		}
 	}
 }
 
@@ -589,35 +616,6 @@ __global__ void __launch_bounds__(64) k_nicam_frames(const __grid_constant__ htv
 		}
 		if(x == 63) dt.nic_ftot[k & (RF - 1)] = (unsigned char) ((wsum[0] + inc) & 3);
 	}
-}
-
-// DQPSK state before each frame: exclusive prefix (mod 4) of the frame totals k0 .. k1,
-// seeded with the state before k0 (valid from the previous batch, 0 at the stream start)
-__global__ void __launch_bounds__(1024) k_nicam_scan(const DevTables dt, int64_t k0, int64_t k1)
-{
-	__shared__ int part[1024];
-	const int t = threadIdx.x;
-	const int64_t n = k1 - k0 + 1, per = (n + 1023) / 1024;
-	const int64_t a = k0 + t * per, b = min(k1 + 1, a + per);
-	const int seed = k0 == 0 ? 0 : dt.nic_fstart[k0 & (RF - 1)];
-	int sum = 0;
-	for(int64_t k = a; k < b; k++) sum += dt.nic_ftot[k & (RF - 1)];
-	part[t] = sum;
-	__syncthreads();
-	for(int o = 1; o < 1024; o <<= 1)
-	{
-		const int add = t >= o ? part[t - o] : 0;
-		__syncthreads();
-		part[t] += add;
-		__syncthreads();
-	}
-	int acc = seed + part[t] - sum;
-	for(int64_t k = a; k < b; k++)
-	{
-		dt.nic_fstart[k & (RF - 1)] = (unsigned char) (acc & 3);
-		acc += dt.nic_ftot[k & (RF - 1)];
-	}
-	if(t == 1023) dt.nic_fstart[(k1 + 1) & (RF - 1)] = (unsigned char) ((seed + part[1023]) & 3);
 }
 
 // ---------------------------------------------------------------------------
@@ -868,6 +866,80 @@ __device__ __forceinline__ unsigned long long kd_div(unsigned long long n, unsig
 	else if(r >= (long long) d) { q++; r -= d; }
 	rem = (unsigned) r;
 	return((unsigned long long) q);
+}
+
+// DQPSK state before each frame k0 + 1 .. k1 + 1 - the state before k0 (valid from the previous batch, 0 at the stream
+// start) plus the frame totals k0 .. k - 1, mod 4 - and, where k_line's sound feed reads them (dt.nic_rec), the records
+// of the symbols of the frames from kr on (ref nicam728.c:342-411). One CTA per frame k0 .. k1.
+// A record holds what the line descriptor's phase B (k_line_desc_a2) works out per symbol: its polarity code and the
+// pulse-table rows of the 6-symbol patterns of symbols s - 5 .. s, with the spacing code of the 5 gaps between them
+// (htv_tables.c); no row at the stream start (s < 5), with more than one gap of the rarer spacing, or without a table.
+#define NR_T 384
+__global__ void __launch_bounds__(NR_T) k_nicam_rec(const __grid_constant__ htv_dparams_t dp, const DevTables dt, int64_t k0, int64_t k1,
+	int64_t kr)
+{
+	__shared__ int red[NR_T / 32];
+	__shared__ long long spos[364 + 5];       // first sample of symbols k 364 - 5 .. k 364 + 363
+	__shared__ unsigned char scd[364 + 5];    // and their polarity codes
+	const int t = threadIdx.x;
+	const int64_t k = k0 + blockIdx.x;
+	int sum = 0;
+	for(int64_t i = k0 + t; i < k; i += NR_T) sum += dt.nic_ftot[i & (RF - 1)];
+	#pragma unroll
+	for(int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xFFFFFFFFu, sum, o);
+	if((t & 31) == 0) red[t >> 5] = sum;
+	__syncthreads();
+	int fs = k0 == 0 ? 0 : dt.nic_fstart[k0 & (RF - 1)];
+	#pragma unroll
+	for(int w = 0; w < NR_T / 32; w++) fs += red[w];
+	fs &= 3;                                  // the state before frame k
+	if(t == 0) dt.nic_fstart[(k + 1) & (RF - 1)] = (unsigned char) ((fs + dt.nic_ftot[k & (RF - 1)]) & 3);
+	if(!dt.nic_rec || k < kr) return;
+
+	const unsigned F = (unsigned) dp.nicam_F, D = (unsigned) dp.nicam_D;
+	const int64_t sb = k * 364 - 5;
+	if(t < 364 + 5)
+	{
+		const int64_t s = sb + t;
+		int cd = 0;
+		long long pos = 0;
+		if(s >= 0)
+		{
+			unsigned rem;
+			pos = (long long) kd_div((unsigned long long) s * F + D - 1, D, 1.0 / (double) D, rem);
+			const int st = t < 5 ? (fs - dt.nic_ftot[(k - 1) & (RF - 1)]) & 3 : fs;     // the state before s's frame
+			const int sy = (st + dt.nic_local[s & (RS - 1)]) & 3;
+			// ref nicam728.c:47,386-391: _syms = {0,1,3,2}; bit0 -> I polarity, bit1 -> Q polarity
+			cd = sy == 2 ? 3 : (sy == 3 ? 2 : sy);
+		}
+		spos[t] = pos;
+		scd[t] = (unsigned char) cd;
+	}
+	__syncthreads();
+	if(t >= 364) return;
+	const int i = t + 5;
+	const int64_t s = sb + i;
+	const int minor_adv = dp.nicam_minor_short ? dp.nicam_sps - 1 : dp.nicam_sps;
+	unsigned rec = (unsigned) scd[i] << 18 | 1u << 20;
+	if(dp.nicam_lut_ok && s >= 5)
+	{
+		// bit j of a pattern = the j-th latest symbol (0 = this one); bit j of gaps: the gap ending at symbol s - j is the
+		// rarer spacing
+		int patI = 0, patQ = 0, gaps = 0;
+		#pragma unroll
+		for(int j = 0; j < 6; j++)
+		{
+			patI |= (scd[i - j] & 1) << j;
+			patQ |= ((scd[i - j] >> 1) & 1) << j;
+			if(j < 5) gaps |= (spos[i - j] - spos[i - j - 1] == minor_adv) << j;
+		}
+		if(__popc(gaps) <= 1)
+		{
+			const int gg = gaps ? __ffs(gaps) : 0;                          // which gap (1 = newest) has the rarer spacing
+			rec = (unsigned) (gg * 64 + patI) | (unsigned) (gg * 64 + patQ) << 9 | (unsigned) scd[i] << 18;
+		}
+	}
+	dt.nic_rec[s & (RS - 1)] = rec;
 }
 
 // A warp takes KD_LINES consecutive lines. Phase A, lane = line: everything that is one value per line or per audio
@@ -2423,8 +2495,8 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 // resident CTAs per SM of a persistent line kernel of MAXT threads
 #define KL_MINB(T) ((T) <= 256 ? KL_B256 : (T) <= 320 ? KL_B320 : KL_B384)
 
-typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, int, int, int16_t *, const int16_t *, int, const int16_t *,
-	const int16_t *);
+typedef void (*KLineFn)(htv_dparams_t, DevTables, const LineR2 *, const LineA2 *, long long, int, int, int16_t *, const int16_t *, int,
+	const int16_t *, const int16_t *);
 // ps: the converted picture store and the subcarrier stage in k_line (encoders without a composite store); not part of
 // the name htv_line_kernel reports
 struct KLine { KLineFn fn; int vf, hq, full, csat, maxt, minb, src, snd, wc, st, ps; };
@@ -2443,10 +2515,18 @@ static const KLine kl_tab[] = {
 	KL_VF(true, false, false, false), KL_VF(false, false, false, false), KL_VF(false, true, false, false),   // 128 | W, a partial last tile, CSAT
 	KL_VF(true, false, false, true), KL_VF(false, false, false, true), KL_VF(false, true, false, true),      // the same, PS
 	KL_VF(true, false, true, false), KL_VF(false, false, true, false),                  // SECAM's SRC form: 128 | W, partial
-	// PAL's VSB + FM + NICAM + complex output and W = 1024 (16 Msps) compiled in, storing int16 or int8 (the HackRF's format)
+	// PAL's VSB + FM + NICAM + complex output and W = 1024 (16 Msps) compiled in, storing int16 or int8 (the HackRF's format).
+	// At 4 CTAs of 256 threads the int16 form's 62 registers (64 allocated) take the whole register file, so the next
+	// call's sound pre-pass, records and raster descriptors run in the tail of k_line and between launches, not inside
+	// it. That is on purpose: bounded to 48 registers, or at 56, the side kernels shared the SMs with k_line at
+	// unpredictable points, and the step got slower and spread (DESIGN.md section 4).
 	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT16),
 	KL_ENTRY(true, true, true, false, 256, false, KL_SND_FM_NICAM, 1024, HTV_TYPE_INT8),
 };
+
+// The k_line forms with the sound stages compiled in derive their sound state per lane (htv_line.cuh KlFeed, FED); every
+// other modulator, the general k_line forms included, reads LineA2
+static inline bool kl_fed(const DevPlan &p) { return((p.path == PATH_LINE || p.path == PATH_SEC_LINE) && p.kl && p.kl->snd >= 0); }
 
 typedef void (*KSecFn)(htv_dparams_t, DevTables, const LineS2 *, int, int, int16_t *, SecScratch);
 struct KSec { KSecFn fn; int full, maxt, minb; };
@@ -2750,7 +2830,7 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 		kl_name(kl, sizeof(kl), *p->kl, type, dp.s_video);
 		// the composite ring and the tap operand where k_line filters: the PS and SRC forms (htv_line.cuh)
 		const bool ring = vf && (p->kl->ps || p->kl->src);
-		p->kl_smem = 2 * sizeof(LineA2) + 2 * sizeof(LineR2) + (ring ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
+		p->kl_smem = (p->kl->snd >= 0 ? 0 : 2 * sizeof(LineA2)) + 2 * sizeof(LineR2) + (ring ? 8 * rowb + sizeof(uint32_t) * MF_ATAB_WORDS : 0) + ntp + 128;
 		// PS forms with S-Video: two rows of chroma, four int16 per thread (htv_line.cuh)
 		if(dp.s_video && p->kl->ps) p->kl_smem += sizeof(short) * 2 * 4 * p->kl_threads;
 	}
@@ -2960,9 +3040,27 @@ extern "C" htv_dev_t *htv_dev_create(const struct htv_tables_t *t, int max_frame
 		dt.nic_ftot = (uint8_t *) dev_zero(d, RF);
 		dt.nic_fstart = (uint8_t *) dev_zero(d, RF);
 	}
+	if(kl_fed(p))
+	{
+		// k_line's sound feed: its records, and what one line adds to each quotient and remainder of its state
+		if(dp.have_fm) dt.seg_rec = (SegRec *) dev_zero(d, sizeof(SegRec) * RA);
+		if(dp.have_nicam) dt.nic_rec = (uint32_t *) dev_zero(d, sizeof(uint32_t) * RS);
+		htv_dparams_t &dw = d->dp;
+		dw.kl_w_kk = dw.W % 32767;
+		dw.kl_w_aq = (uint32_t) (((uint64_t) dw.W * HTV_AUDIO_RATE) / (uint64_t) dw.rate);
+		dw.kl_w_ar = (uint32_t) (((uint64_t) dw.W * HTV_AUDIO_RATE) % (uint64_t) dw.rate);
+		if(dw.have_nicam)
+		{
+			dw.kl_w_cc = dw.W % dw.nicam_cc_len;
+			dw.kl_w_sq = (uint32_t) (((uint64_t) dw.W * (uint64_t) dw.nicam_D) / (uint64_t) dw.nicam_F);
+			dw.kl_w_sr = (uint32_t) (((uint64_t) dw.W * (uint64_t) dw.nicam_D) % (uint64_t) dw.nicam_F);
+		}
+	}
 	if(!dt.codes || !d->h_map || d->alloc_failed || cudaGetLastError() != cudaSuccess) return(create_fail(d, err, errlen, "device allocation failed"));
 	d->fm_jc = -1;
 	d->nic_kc = 0;
+	d->fm_jr = -2;
+	d->nic_kr = -1;
 
 	const int W = dp.W;
 	const bool secam = dp.colour_mode == HTV_SECAM;
@@ -3308,9 +3406,9 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	if(m1 <= m0) return(HTV_OK);
 	// everything the caller queued so far (PCM uploads) precedes the pre-pass, which runs on the
 	// side stream so that it overlaps the raster kernels of the same call
-	// Fused line kernel: the pre-pass chain and the sound descriptors touch nothing the caller's stream produces - the
-	// PCM comes up on the upload stream (ev_up), the descriptors are double-buffered - so they do not wait for the
-	// previous call's line kernel but run beside its tail (HTV_AHEAD=0: in the caller's stream order, for A/B)
+	// Fused line kernel: the pre-pass chains and their records touch nothing the caller's stream produces - the PCM comes
+	// up on the upload stream (ev_up), the rings hold two calls - so they do not wait for the previous call's line kernel
+	// but run beside its tail (HTV_AHEAD=0: in the caller's stream order, for A/B)
 	if(d->ahead) CK(cudaStreamWaitEvent(d->side, d->ev_up, 0));
 	else
 	{
@@ -3319,6 +3417,11 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 	}
 	d->side_armed = 1;
 	cudaStream_t st = d->side;
+	// the records of k_line's sound feed, where the plan's k_line reads them (a sample type set after htv_dev_create can
+	// choose a general form, which reads LineA2)
+	const bool fed = kl_fed(d->plan);
+	DevTables dtr = d->dt;
+	if(!fed) { dtr.seg_rec = NULL; dtr.nic_rec = NULL; }
 	if(dp.have_fm)
 	{
 		const int64_t jA = d->fm_jc;                               // restart from the last valid prefix entry
@@ -3336,9 +3439,10 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 			k_fm_limit<<<(unsigned) ((n + 127) / 128), 128, 0, st>>>(dp, d->dt, jA, jB);
 			const unsigned nb = (unsigned) ((n + SCAN_BLK - 1) / SCAN_BLK);
 			k_fm_scan_local<<<nb, SCAN_T, 0, st>>>(d->dt, jA, jB);
-			k_fm_scan_fix<<<nb, SCAN_T, 0, st>>>(d->dt, jA, jB);
+			k_fm_scan_fix<<<nb, SCAN_T, 0, st>>>(dtr, jA, jB, d->fm_jr);
 			d->launches += 3;
 			d->fm_jc = jB;
+			if(dtr.seg_rec) d->fm_jr = jB;
 		}
 	}
 	if(dp.have_nicam)
@@ -3352,15 +3456,22 @@ extern "C" int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void 
 		if(k_lo > d->nic_kc) k_lo = d->nic_kc;                     // keep the frame-start chain contiguous
 		if(k_hi - k_lo + 2 >= RF / 2 || (k_hi - k_lo + 2) * 364 >= RS / 2) return(HTV_ERROR);
 		k_nicam_frames<<<(unsigned) (k_hi - k_lo + 1), 64, 0, st>>>(dp, d->dt, k_lo);
-		k_nicam_scan<<<1, 1024, 0, st>>>(d->dt, k_lo, k_hi);
+		k_nicam_rec<<<(unsigned) (k_hi - k_lo + 1), NR_T, 0, st>>>(dp, dtr, k_lo, k_hi, d->nic_kr + 1);
 		d->launches += 2;
 		d->nic_kc = k_hi;                                          // fstart[k_hi] is valid; recompute from there next time
+		if(dtr.nic_rec && k_hi > d->nic_kr) d->nic_kr = k_hi;
+	}
+	if(fed)
+	{
+		// k_line reads the records (and, for AM, the PCM): its wait for the sound is a wait for the two chains
+		CK(cudaEventRecord(d->ev_audio, d->side));
+		if(dp.have_nicam) CK(cudaEventRecord(d->ev_nic, d->side2));
 	}
 	CK(cudaGetLastError());
 	return(HTV_OK);
 }
 
-// The sound descriptors of lines line0 .. line0 + n - 1, each half on the side stream of the pre-pass chain it depends
+// The sound descriptors of lines line0 .. line0 + n - 1 (every modulator but the k_line forms kl_fed feeds), each half on the side stream of the pre-pass chain it depends
 // on; ev_audio and ev_nic mark the two halves done. The fused line kernel's buffers are two, so that the next call's
 // descriptors may be written while this call's line kernel runs: with HTV_AHEAD they wait for the line kernel that last
 // read their buffer, not for the caller's stream. Every other path's wait for this call's place in the caller's stream.
@@ -3410,7 +3521,7 @@ static int desc_reserve(htv_dev_t *d, int n, cudaStream_t st)
 	static_assert(sizeof(LineS2) == sizeof(LineR2), "one raster descriptor buffer holds either");
 	if(p.path != PATH_RS) CK(cudaMalloc(&d->d_desc_r, bufs * sizeof(LineR2) * ((size_t) n + p.before + p.after)));
 	// + 1: FM video's fill line (fm_skip)
-	if(p.path != PATH_RASTER) CK(cudaMalloc(&d->d_desc_a2, bufs * sizeof(LineA2) * ((size_t) n + 1)));
+	if(p.path != PATH_RASTER && !kl_fed(p)) CK(cudaMalloc(&d->d_desc_a2, bufs * sizeof(LineA2) * ((size_t) n + 1)));
 	if(d->dt.filt)
 	{
 		d->vf_cap = vf_list_bound(n + p.before + p.after, p.before, d->dp.lines, HTV_OV_CAP);
@@ -3599,9 +3710,9 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, i
 	const int fm_skip = dp.have_fmv && dp.fmv_ntaps > 0 && line0 == 0 ? 1 : 0;
 	if(desc_reserve(d, nlines, st) != HTV_OK || (r && desc_reserve(r, nlines, st) != HTV_OK)) return(HTV_ERROR);
 	void *desc_r;                                   // entry i <-> line line0 - before + i
-	LineA2 *la2;                                    // la2[i] <-> line line0 - fm_skip + i
+	LineA2 *la2 = NULL;                             // la2[i] <-> line line0 - fm_skip + i
 	if(launch_desc_r(d, r ? r : d, line0, nlines, st, &desc_r) != HTV_OK ||
-		launch_desc_a2(d, line0 - fm_skip, nlines + fm_skip, st, &la2) != HTV_OK) return(HTV_ERROR);
+		(!kl_fed(p) && launch_desc_a2(d, line0 - fm_skip, nlines + fm_skip, st, &la2) != HTV_OK)) return(HTV_ERROR);
 	int sub = p.path == PATH_LINE ? nlines : d->sub_lines;
 	if(r && r->sub_lines < sub) sub = r->sub_lines;
 	// where the split and FM-video modulators read the composite scratch: line b of the sub-batch at row b + 1
@@ -3662,8 +3773,8 @@ extern "C" int htv_dev_render_lines(htv_dev_t *d, htv_dev_t *r, int64_t line0, i
 			int run;
 			const int grid = persistent_grid(n, d->kl_ctas, &run);
 			const bool line = p.path == PATH_LINE;
-			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, line ? (const LineR2 *) desc_r : NULL, la2 + done, n, run,
-				o, acc, acc_rows, line ? NULL : d->d_comp, line ? NULL : d->d_compq);
+			p.kl->fn<<<grid, p.kl_threads, p.kl_smem, st>>>(dp, d->dt, line ? (const LineR2 *) desc_r : NULL, la2 ? la2 + done : NULL,
+				(line0 + done) * (long long) dp.W + dp.shift, n, run, o, acc, acc_rows, line ? NULL : d->d_comp, line ? NULL : d->d_compq);
 			if(line)
 			{
 				// this call's descriptor buffers are free again once ev_kl has passed; the next call takes the other two

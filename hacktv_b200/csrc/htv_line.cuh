@@ -16,8 +16,7 @@
 // samples in the layout the m16n8k32 accumulators have anyway: lane = 4g + t holds x = 128 tile + 32 t + g + 8 j,
 // j = 0..3 (htv_mma_fir.h: mf_out_x). Both filters leave their results in exactly the registers the next
 // stage needs - no exchange through shared memory, and all four samples of a lane fall into one 32-sample
-// block, which is what the per-line sound descriptors are indexed by: the sound carriers and mixers are htv_sound.cuh's
-// with S = 8. Loads and stores with a stride of 8 samples between a lane's values are still sector-exact (8 lanes x 4
+// block: the sound carriers and mixers are htv_sound.cuh's with S = 8, fed per lane (KlFeed below). Loads and stores with a stride of 8 samples between a lane's values are still sector-exact (8 lanes x 4
 // bytes = one 32-byte sector).
 
 #define KL_LEAD   MF_LEAD   // composite row: byte i = sample i - 32 of the line (htv_mma_fir.h pitched row)
@@ -74,11 +73,23 @@ __device__ __forceinline__ void kl_vfilter(const unsigned char *ph, int RB, cons
 // (`acc`, int16 in the output layout) still adds in int16 with wrap-around; the conversion is the last step, as the
 // reference's file sink converts what the video stage handed it. A lane stores each of its samples on its own (1, 2,
 // 4 or 8 bytes); the eight lanes g = 0..7 of a t still cover one contiguous run of the line per j.
-template<bool FULL, int SND, int ST>
-__device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la,
-	int W, int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
+// the mixers from the line's sound descriptor or from the lane state (FED)
+template<int SND>
+__device__ __forceinline__ void kl_mix8(const htv_dparams_t &dp, const DevTables &dt, const LineA2 *la, int xb, int (&oi)[4], int (&oq)[4])
 {
 	kl_mix<SND, 8>(dp, dt, la, xb, oi, oq);
+}
+template<int SND>
+__device__ __forceinline__ void kl_mix8(const htv_dparams_t &dp, const DevTables &dt, const KlLane &L, int xb, int (&oi)[4], int (&oq)[4])
+{
+	kl_mix_lane<SND, 8>(dp, dt, L, oi, oq);
+}
+
+template<bool FULL, int SND, int ST, typename IN>
+__device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const DevTables &dt, const IN &in,
+	int W, int xb, int row, int (&oi)[4], int (&oq)[4], int16_t *out, const int16_t *acc)
+{
+	kl_mix8<SND>(dp, dt, in, xb, oi, oq);
 	const size_t lbase = (size_t) row * (size_t) W;
 	if constexpr(ST != HTV_TYPE_INT16)
 	{
@@ -122,6 +133,161 @@ __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const Dev
 	}
 }
 
+// ---- k_line's sound feed ---------------------------------------------------------------------------------------
+// A lane's samples are xb + 8 j of every line, so the audio-clock index m = L W + shift + xb of its first sample grows by
+// exactly W from one line to the next. The sound state is a closed form of m: the audio index in effect
+// j = floor(32000 (m + 1) / rate) - 1, the NICAM symbol in effect s = floor(m D / F), m mod 32767 and m mod nicam_cc_len.
+// A CTA sets them up once by exact 64-bit division (kd_div) and then advances each quotient and remainder by the
+// increments of one line (htv_dparams_t kl_w_*). What varies per audio sample or per symbol comes from the records the
+// pre-pass chains write - dt.seg_rec (k_fm_scan_fix) and dt.nic_rec (k_nicam_rec) - loaded where the line's lane
+// state is built (kl_lane_feed), so that no record is held in registers from one line to the next.
+struct KlFeed {
+	unsigned aq, ar;            // 32000 (m + 1) = aq rate + ar: aq = j + 1 (mod 2^32), the slot of j's record
+	unsigned sq, sr;            // m D = sq F + sr: sq = s (mod 2^32); sr / D samples into symbol s
+	int kk, cc;                 // m mod 32767, m mod nicam_cc_len
+	ulonglong2 seg;             // record of audio index j: B(j), angle step ... (kl_feed_load)
+	float2 rot;                 // ... and (cos, sin) of 8 steps
+	unsigned nA, nB;            // records of symbols s and s + 1
+};
+
+template<int SND>
+__device__ __forceinline__ void kl_feed_load(const htv_dparams_t &dp, const DevTables &dt, KlFeed &f)
+{
+	if(KL_HAS(SND, KL_FM, dp.have_fm))
+	{
+		const SegRec *r = dt.seg_rec + (f.aq & (RA - 1));
+		f.seg = __ldg(&r->ba);
+		f.rot = __ldg(&r->rot);
+	}
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
+	{
+		f.nA = __ldg(dt.nic_rec + (f.sq & (RS - 1)));
+		f.nB = __ldg(dt.nic_rec + ((f.sq + 1) & (RS - 1)));
+	}
+}
+
+// the feed of audio-clock index m (>= 0)
+template<int SND>
+__device__ __forceinline__ void kl_feed_init(const htv_dparams_t &dp, const DevTables &dt, KlFeed &f, long long m)
+{
+	unsigned rem;
+	kd_div((unsigned long long) m, 32767u, 1.0 / 32767.0, rem);
+	f.kk = (int) rem;
+	if(KL_HAS(SND, KL_FM, dp.have_fm) || KL_HAS(SND, KL_AM, dp.have_am))
+	{
+		f.aq = (unsigned) kd_div((unsigned long long) (m + 1) * HTV_AUDIO_RATE, (unsigned) dp.rate, 1.0 / (double) dp.rate, rem);
+		f.ar = rem;
+	}
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
+	{
+		f.sq = (unsigned) kd_div((unsigned long long) m * (unsigned) dp.nicam_D, (unsigned) dp.nicam_F, 1.0 / (double) dp.nicam_F, rem);
+		f.sr = rem;
+		kd_div((unsigned long long) m, (unsigned) dp.nicam_cc_len, 1.0 / (double) dp.nicam_cc_len, rem);
+		f.cc = (int) rem;
+	}
+}
+
+// the feed W samples on (the lane's first sample on the next line)
+template<int SND>
+__device__ __forceinline__ void kl_feed_next(const htv_dparams_t &dp, const DevTables &dt, KlFeed &f)
+{
+	f.kk += dp.kl_w_kk;
+	if(f.kk >= 32767) f.kk -= 32767;
+	if(KL_HAS(SND, KL_FM, dp.have_fm) || KL_HAS(SND, KL_AM, dp.have_am))
+	{
+		f.aq += dp.kl_w_aq; f.ar += dp.kl_w_ar;
+		if(f.ar >= (unsigned) dp.rate) { f.ar -= (unsigned) dp.rate; f.aq++; }
+	}
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
+	{
+		f.sq += dp.kl_w_sq; f.sr += dp.kl_w_sr;
+		if(f.sr >= (unsigned) dp.nicam_F) { f.sr -= (unsigned) dp.nicam_F; f.sq++; }
+		f.cc += dp.kl_w_cc;
+		if(f.cc >= dp.nicam_cc_len) f.cc -= dp.nicam_cc_len;
+	}
+}
+
+// the sound stage's lane state from the feed at audio-clock index m (the segment start st(j) = m - floor(ar / 32000):
+// the record of j = -1 is stored one step back, so that the same form holds at the stream start, where st = 0).
+// PART: which of L's fields - 1 the FM and AM carriers' and kk, 2 NICAM's, 4 the offset mixer's (kl_sound)
+template<int SND, int PART>
+__device__ __forceinline__ void kl_lane_feed(const htv_dparams_t &dp, const DevTables &dt, KlFeed f, long long m, KlLane &L)
+{
+	kl_feed_load<SND>(dp, dt, f);
+	if(PART & 1)
+	{
+		L.kk = f.kk;
+		L.nb = 0x7FFFFFFF;
+	}
+	const bool fm = (PART & 1) && KL_HAS(SND, KL_FM, dp.have_fm), am = (PART & 1) && KL_HAS(SND, KL_AM, dp.have_am);
+	if(fm || am)
+	{
+		const int nb = (int) (((unsigned) dp.rate - f.ar + HTV_AUDIO_RATE - 1) / HTV_AUDIO_RATE);   // first sample of j + 1
+		if(nb <= 24) L.nb = nb;
+		if(fm)
+		{
+			L.angA = f.seg.y;
+			L.phA = f.seg.x + f.seg.y * (unsigned long long) (f.ar / HTV_AUDIO_RATE + 1);
+			L.rot = f.rot;
+			L.angB = L.angA; L.phB = L.phA;
+			if(nb <= 24)
+			{
+				const ulonglong2 b = __ldg(&dt.seg_rec[(f.aq + 1) & (RA - 1)].ba);
+				L.angB = b.y;
+				L.phB = b.x - b.y * (unsigned long long) (nb - 1);
+			}
+		}
+		if(am)
+		{
+			const bool neg = (unsigned long long) HTV_AUDIO_RATE * (unsigned long long) (m + 1) < (unsigned long long) dp.rate;   // j < 0
+			L.amA = (pcm_mono(dt, neg ? -1 : (int64_t) (f.aq - 1), dp.volume) + 32768) / 2;
+			L.amB = (pcm_mono(dt, (int64_t) f.aq, dp.volume) + 32768) / 2;
+			L.phM = dp.am_ang * (unsigned long long) (m + 1);
+		}
+	}
+	if((PART & 2) && KL_HAS(SND, KL_NIC, dp.have_nicam))
+	{
+		const unsigned D = (unsigned) dp.nicam_D;
+		const int off = (int) (f.sr / D), dist = (int) (((unsigned) dp.nicam_F - f.sr + D - 1) / D);   // s started off samples ago, s + 1 starts at dist
+		L.nbs = dist;
+		L.niA = (int) (f.nA & 511u) * dp.nicam_sps + off; L.nqA = (int) ((f.nA >> 9) & 511u) * dp.nicam_sps + off;
+		L.niB = (int) (f.nB & 511u) * dp.nicam_sps - dist; L.nqB = (int) ((f.nB >> 9) & 511u) * dp.nicam_sps - dist;
+		L.gen = !dp.nicam_lut_ok || dp.nicam_sps - 1 < 32 || ((f.nA >> 20) & 1u) || (dist <= 24 && ((f.nB >> 20) & 1u));
+		L.cc = f.cc;
+	}
+	if(PART & 4)
+	{
+		L.kk = f.kk;
+		L.m = m;
+		L.offph = dp.offset_phase0 + dp.offset_ang * (unsigned long long) (m + 1 - 32767);
+	}
+}
+
+// the generic NICAM sum of the samples m + 8 j: the symbols whose pulse covers a sample, from the newest started at or
+// before it (symbol sx, rx / D samples ago) back, their polarities from the records
+__device__ __forceinline__ void kl_nic_generic_feed(const htv_dparams_t &dp, const DevTables &dt, const KlFeed &f, long long m,
+	const short *ntp, int (&bi)[4], int (&bq)[4])
+{
+	const unsigned F = (unsigned) dp.nicam_F, D = (unsigned) dp.nicam_D;
+	#pragma unroll
+	for(int j = 0; j < 4; j++)
+	{
+		unsigned rx = f.sr + 8u * j * D;
+		const unsigned sx = f.sq + rx / F;
+		rx %= F;
+		bi[j] = 0; bq[j] = 0;
+		for(int cnd = 0; cnd < NIC_CAND; cnd++)
+		{
+			const unsigned d = (rx + cnd * F) / D;                      // samples since symbol sx - cnd started
+			if((long long) d > m + 8 * j) break;                        // before the stream start
+			const int sy = (int) (__ldg(dt.nic_rec + ((sx - cnd) & (RS - 1))) >> 18) & 3;
+			const int r = ntp[d + NIC_TPAD];                            // the table is zero outside the pulse
+			bi[j] += (sy & 1) ? r : -r;
+			bq[j] += (sy & 2) ? r : -r;
+		}
+	}
+}
+
 // cp.async: 16 bytes global -> shared without passing through registers
 __device__ __forceinline__ void kl_cp16(void *dst_smem, const void *src)
 {
@@ -136,14 +302,21 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 // The forms with a video filter and a composite store (FS: VF, not PS, not SRC) do not filter: k_vf_rows filtered each
 // line's three composite rows and overlays once, into the filtered store (a row per line of each slot and phase) or,
 // for the lines whose filter window leaves one frame's rows or meets an overlay, into the call's own rows. Per
-// iteration q they load line q + 1's filtered I | Q (R1), and give line q its sound carriers and store it (M).
+// iteration q they load line q + 1's filtered I | Q (R1), and give line q its sound carriers and store it (M). They read
+// the raster descriptor's pic a line ahead of R1 by a uniform load; with the sound state fed per lane (FED, below) that
+// is their only per-line value, and their warps share nothing per line and meet at no barrier.
 //
 // Every other form, per iteration q (one scan line), runs
 //   R2(q)   VBI overlay on the values fetched earlier, composite row q mod 4                  | __syncthreads
 //   R1(q+1) the composite row of the NEXT line is loaded here ...
 //   M(q-1)  ... and arrive while line q - 1 (whose right-hand halo R2(q) has just written) is filtered (mma),
 //           gets its sound carriers and is stored.
-// The line descriptors (LineR2 of q + 1, LineA2 of q - 1) come in by cp.async at the top of the iteration.
+// The raster descriptor of line q + 1 and, unless FED, the sound descriptor of the line modulated come in by cp.async at
+// the top of the iteration.
+// FED: the forms with the sound stages compiled in (SND >= 0) derive each lane's sound state from its audio-clock index
+// (KlFeed), set up once per CTA and advanced by W per line, instead of reading LineA2. The general forms (SND = -1)
+// keep reading LineA2: with every stage a run-time flag, the feed's state and arithmetic cost them more registers and
+// time than the descriptor does (at W = 1280, 320 threads: k_line 0.385 against 0.217 ms per 64 frames on an H100).
 // One barrier per line, so the ring has 4 rows: a warp that is through M(q - 1) may run on into R2(q + 1), before the
 // next barrier, while another warp is still reading line q - 1's row. R2(q + 1) writes line q + 1's row, the right
 // halo of line q's and the left halo of line q + 2's; with 4 rows none of them is line q - 1's.
@@ -165,17 +338,19 @@ __device__ __forceinline__ void kl_cp_wait() { asm volatile("cp.async.wait_all;"
 template<bool VF, bool HASQ, bool FULL, bool CSAT, int MAXT, int MINB, bool SRC = false, int SND = -1, int WC = 0, int ST = HTV_TYPE_INT16,
 	bool PS = false>
 __global__ void __launch_bounds__(MAXT, MINB)
-k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap,
+k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR2 *lrp, const LineA2 *lap, long long mf,
 	int nlines, int run, int16_t *out, const int16_t *acc, int acc_rows, const int16_t *src = nullptr, const int16_t *srcq = nullptr)
 {
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	// FS: the filtered store holds each line's filter output (k_vf_rows); RING: the filter runs here, on the ring
-	constexpr bool FS = VF && !PS && !SRC, RING = VF && !FS;
+	constexpr bool FS = VF && !PS && !SRC, RING = VF && !FS, FED = SND >= 0;
 	const int W = WC ? WC : dp.W;
 	const int RB = kl_row_bytes(W);
-	// descriptors x2 | RING: [row 0..3][hi, lo] composite planes, FIR taps | NICAM pulse | PS, S-Video: chroma [row 0..1][j][thread]
+	// lap: the sound descriptors (not FED); mf: the audio-clock index of relative line 0's first sample (line0 W + shift, FED)
+	// sound descriptors x2 (not FED) | raster descriptors x2 | RING: [row 0..3][hi, lo] composite planes, FIR taps | NICAM
+	// pulse | PS, S-Video: chroma [row 0..1][j][thread]
 	LineA2 *sla = reinterpret_cast<LineA2 *>(smem_raw);
-	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + 2);
+	LineR2 *slr = reinterpret_cast<LineR2 *>(sla + (FED ? 0 : 2));
 	unsigned char *rows = reinterpret_cast<unsigned char *>(slr + 2);
 	uint4 *atab = reinterpret_cast<uint4 *>(rows + (RING ? 8 * RB : 0));  // [k-step][I hi, I lo, Q hi, Q lo][lane]
 	short *ntp = reinterpret_cast<short *>(atab + (RING ? MF_ATAB_WORDS / 4 : 0));
@@ -199,14 +374,22 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 		int4 *dst = reinterpret_cast<int4 *>(ntp);
 		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
 	}
-	if(!SRC && tid < 4) reinterpret_cast<int4 *>(slr + (q0 & 1))[tid] = __ldg(reinterpret_cast<const int4 *>(lrp + q0 + 1) + tid);
+	if(!SRC && !FS && tid < 4) reinterpret_cast<int4 *>(slr + (q0 & 1))[tid] = __ldg(reinterpret_cast<const int4 *>(lrp + q0 + 1) + tid);
 	__syncthreads();
+	// FS: pic of the line R1 loads next (q0, then q0 + 1 ...), and of the one after it
+	long long fpic = FS ? __ldg(&lrp[q0 + 1].pic) : 0;
+	long long fpn = FS && q0 + 1 <= q1 ? __ldg(&lrp[q0 + 2].pic) : 0;
+	const bool snd = FED && KL_HAS(SND, KL_FM, dp.have_fm) || KL_HAS(SND, KL_AM, dp.have_am) || KL_HAS(SND, KL_NIC, dp.have_nicam) ||
+		KL_HAS(SND, KL_OFF, dp.have_offset);
+	const long long mx0 = mf + xb;                                          // the lane's first sample on relative line 0
+	KlFeed fd;
+	if(snd) kl_feed_init<SND>(dp, dt, fd, mx0 + (long long) a * W);
 
 	// PS: the span the chroma low-pass reaches (taps <= 17: 8 samples either side of the picture); the store is zero outside
 	const bool in_chroma = xb + 24 >= dp.active_left - 8 && xb < dp.active_left + dp.active_width + 8;
 	const bool in_burst = xb + 24 >= dp.burst_left && xb < dp.burst_left + dp.burst_width;
 	const int fo0 = mf_b_offset(nt, 0, lane);
-	constexpr int NA16 = (int) (sizeof(LineA2) / 16);
+	constexpr int NA16 = FED ? 0 : (int) (sizeof(LineA2) / 16);
 
 	// loads of line q issued one phase early: the line's composite row (int16 x 4); FS: the line's filtered I | Q << 16
 	// (x 4), from the filtered store or, for the lines k_line_desc_r listed (pic < 0), from the call's rows at the list
@@ -216,7 +399,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	#define KL_R1(QQ) do { \
 		if(FS) \
 		{ \
-			const long long pic_ = slr[(QQ) & 1].pic; \
+			const long long pic_ = fpic; \
 			const uint32_t *fp_ = (pic_ >= 0 ? dt.filt + pic_ : dt.vfx + (size_t) (-1 - pic_) * W) + xb; \
 			_Pragma("unroll") for(int j = 0; j < 4; j++) px[j] = (FULL || xb + 8 * j < W) ? __ldg(fp_ + 8 * j) : 0u; \
 			break; \
@@ -244,12 +427,11 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	for(int q = q0; q <= q1; q++, r4 = (r4 + 1) & 3)
 	{
 		const int mrow = RING ? q - 1 : q;                                  // the line modulated in this iteration
-		// ---- descriptors of the next raster line and of the line modulated below -> shared memory -----
-		if(tid < 4) { if(!SRC && q + 1 <= q1) kl_cp16(reinterpret_cast<int4 *>(slr + ((q + 1) & 1)) + tid, reinterpret_cast<const int4 *>(lrp + q + 2) + tid); }
+		// ---- the raster descriptor of the next line -> shared memory ------------------------------------------
+		if(tid < 4) { if(!SRC && !FS && q + 1 <= q1) kl_cp16(reinterpret_cast<int4 *>(slr + ((q + 1) & 1)) + tid, reinterpret_cast<const int4 *>(lrp + q + 2) + tid); }
 		else if(tid < 4 + NA16) { if(mrow >= a) kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + (tid - 4), reinterpret_cast<const int4 *>(lap + mrow) + (tid - 4)); }
-		// a CTA narrower than 4 + NA16 threads (one warp: W <= 128) copies the rest of the descriptor in further passes;
-		// the forms with the width compiled in have 256 threads and need none
-		if(!WC && (int) blockDim.x < 4 + NA16 && mrow >= a)
+		// a CTA narrower than 4 + NA16 threads (one warp: W <= 128) copies the rest of the sound descriptor in further passes
+		if(!FED && (int) blockDim.x < 4 + NA16 && mrow >= a)
 			for(int i = (int) blockDim.x - 4 + tid; i < NA16; i += blockDim.x)
 				kl_cp16(reinterpret_cast<int4 *>(sla + (mrow & 1)) + i, reinterpret_cast<const int4 *>(lap + mrow) + i);
 
@@ -345,11 +527,19 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 				}
 			}
 		}
-		if(tid < 4 + NA16 || (!WC && (int) blockDim.x < 4 + NA16)) kl_cp_wait();
-		__syncthreads();                                                    // rows of line q, descriptors of q + 1 and of mrow
+		if(!FS || !FED)
+		{
+			if(tid < 4 + NA16 || (!FED && (int) blockDim.x < 4 + NA16)) kl_cp_wait();
+			__syncthreads();                                                // rows of line q, the descriptors of q + 1 and of mrow
+		}
 
 		// ---- R1: the next line's values start their way here -------------------------
-		if(q + 1 <= q1) KL_R1(q + 1);
+		if(q + 1 <= q1)
+		{
+			fpic = fpn;
+			KL_R1(q + 1);
+			if(FS && q + 2 <= q1) fpn = __ldg(&lrp[q + 3].pic);
+		}
 		if(mrow < a) continue;
 
 		int oi[4], oq[4];
@@ -379,9 +569,24 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 					else oq[j] += (FULL || xb + 8 * j < W) ? (int) __ldg(qp + 8 * j) : 0;
 				}
 			}
-			const LineA2 *la = sla + (mrow & 1);
-			kl_sound<SND, 8>(dp, dt, la, ntp, xb, oi, oq);
-			kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
+			if(!FED)
+			{
+				const LineA2 *la = sla + (mrow & 1);
+				kl_sound<SND, 8>(dp, dt, la, ntp, xb, oi, oq);
+				kl_post_store<FULL, SND, ST>(dp, dt, la, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
+				continue;
+			}
+			const long long m = mx0 + (long long) mrow * W;
+			// the FM and AM carriers, NICAM, the mixers: each part's state built right before it runs
+			KlLane L;
+			const auto gen = [&](int (&bi)[4], int (&bq)[4]) { kl_nic_generic_feed(dp, dt, fd, m, ntp, bi, bq); };
+			kl_lane_feed<SND, 1>(dp, dt, fd, m, L);
+			kl_sound_lane<SND, 8, false, 1>(dp, dt, L, oi, oq, gen);
+			kl_lane_feed<SND, 2>(dp, dt, fd, m, L);
+			kl_sound_lane<SND, 8, false, 2>(dp, dt, L, oi, oq, gen);
+			kl_lane_feed<SND, 4>(dp, dt, fd, m, L);
+			if(snd) kl_feed_next<SND>(dp, dt, fd);
+			kl_post_store<FULL, SND, ST>(dp, dt, L, W, xb, mrow, oi, oq, out, mrow < acc_rows ? acc : NULL);
 		}
 	}
 	#undef KL_R1

@@ -1,9 +1,13 @@
 // hacktv_b200 - the sound carriers and the post-modulation mixers (included by htv_kernels.cu), for the fused line kernel
-// (htv_line.cuh) and for the split and FM-video modulators alike. Both read the per-line sound descriptor LineA2
-// (k_line_desc_a2) and work on four samples per thread, S apart:
+// (htv_line.cuh) and for the split and FM-video modulators alike, on four samples per thread, S apart:
 //   S = 8: k_line's lane layout (x = xb + 8 j, the m16n8k32 accumulator layout, htv_mma_fir.h: mf_out_x);
 //   S = 1: four consecutive samples (k_mod, k_mod_tma, k_mod_mma, k_fmv_base, k_fmv_mod).
-// Either way all four samples fall into one 32-sample block, which is what the descriptor is indexed by.
+// Either way all four samples fall into one 32-sample block. kl_sound / kl_mix read the per-line sound descriptor
+// LineA2 (k_line_desc_a2), which the descriptor is indexed by; kl_sound_lane / kl_mix_lane run the same arithmetic on
+// a lane state (KlLane) that the k_line forms with the sound stages compiled in derive per lane (htv_line.cuh KlFeed).
+// Two entries rather than one fed two ways: built from LineA2 through a KlLane, the general forms of k_line and the
+// split modulators held the state in registers instead of reading it from shared memory where they use it, and the
+// 320-thread k_line forms spilled 120-340 bytes.
 
 #define KL_BIAS   2048      // NICAM pulse-table index bias (LineA2.symb)
 
@@ -197,6 +201,136 @@ __device__ __forceinline__ void kl_sound(const htv_dparams_t &dp, const DevTable
 	}
 }
 
+// ---- the same carriers from a lane state ---------------------------------------------------------------------------
+// The state of the carriers at the thread's first sample u = 0 (k_line: KlFeed, htv_line.cuh). A is the audio segment /
+// NICAM symbol in effect at u = 0, B the next one; at most one boundary of either kind falls among the four samples.
+struct KlLane {
+	unsigned long long phA, angA, phB, angB;  // FM: phase at u = 0 in segment A / B, and per sample
+	float2 rot;                               // FM: (cos, sin) of 8 angle steps of A
+	int nb;                                   // B is in effect from u = nb on (> 0; > 3 S: on none of the samples)
+	int kk;                                   // audio-clock index of u = 0, mod 32767
+	unsigned long long phM;                   // AM: carrier phase at u = 0
+	int amA, amB;                             // AM: (sample + 32768) / 2 of A and B
+	int gen;                                  // NICAM: the generic sum instead of the pulse table
+	int niA, nqA, niB, nqB;                   // NICAM: pulse-table index (I, Q) of u = 0 under symbol A / B
+	int nbs;                                  // NICAM: B is in effect from u = nbs on
+	int cc;                                   // NICAM: carrier-table index of u = 0
+	long long m;                              // offset mixer: audio-clock index of u = 0 ...
+	unsigned long long offph;                 // ... and the mixer's phase there
+};
+
+// the carriers from a lane state; nic_generic(bi, bq) gives the generic NICAM sum of the four samples (stream start,
+// symbols without a pulse-table row, rates where a symbol is 32 samples or shorter). PART: 1 the FM and AM carriers
+// (fields nb .. amB of L), 2 NICAM (gen .. cc), 3 both - k_line fills and runs the two parts one after the other, so
+// that the state of only one of them is held at a time.
+template<int SND, int S, bool PRECISE = false, int PART = 3, typename G>
+__device__ __forceinline__ void kl_sound_lane(const htv_dparams_t &dp, const DevTables &dt, const KlLane &L, int (&oi)[4], int (&oq)[4],
+	G nic_generic)
+{
+	const bool fm = (PART & 1) && KL_HAS(SND, KL_FM, dp.have_fm), am = (PART & 1) && KL_HAS(SND, KL_AM, dp.have_am);
+	if(fm || am)
+	{
+		const int nb = L.nb;
+		// amplitude of the reference's Q31 phasor kk + 1 multiplications after a renormalisation
+		const float kf = (float) (L.kk + 1);
+		const bool mixed = S == 1 || nb <= 3 * S || L.kk + 3 * S + 1 > 32767;
+		if(fm)
+		{
+			if(!mixed)
+			{
+				const unsigned long long ph = L.phA;
+				const float2 rot = L.rot;
+				float sn, cs;
+				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);   // pi / 2^31
+				float amp = 32767.99998f - kf * 1.52587890625e-5f;
+				#pragma unroll
+				for(int j = 0; j < 4; j++)
+				{
+					oi[j] += (__float2int_rd(amp * cs) * dp.fm_level) >> 15;
+					oq[j] += (__float2int_rd(amp * sn) * dp.fm_level) >> 15;
+					const float c2 = __fmaf_rn(cs, rot.x, -(sn * rot.y)), s2 = __fmaf_rn(sn, rot.x, cs * rot.y);
+					cs = c2; sn = s2;
+					amp -= (float) S * 1.52587890625e-5f;
+				}
+			}
+			else
+			{
+				unsigned long long phA = L.phA, phB = L.phB;
+				const unsigned long long stA = L.angA * S, stB = L.angB * S;
+				float kq = kf;
+				#pragma unroll
+				for(int j = 0; j < 4; j++)
+				{
+					const unsigned long long ph = S * j >= nb ? phB : phA;
+					if(kq > 32767.0f) kq -= 32767.0f;
+					if(PRECISE)
+					{
+						double sn, cs;
+						sincospi((double) (long long) ph * 1.0842021724855044e-19, &sn, &cs);     // 2 / 2^64
+						const double amp = 32767.999984741211 - (double) kq * 1.52587890625e-5;
+						oi[j] += (min((int) floor(amp * cs), 32767) * dp.fm_level) >> 15;
+						oq[j] += (min((int) floor(amp * sn), 32767) * dp.fm_level) >> 15;
+					}
+					else
+					{
+						const float amp = 32767.99998f - kq * 1.52587890625e-5f;
+						float sn, cs;
+						__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
+						oi[j] += (__float2int_rd(amp * cs) * dp.fm_level) >> 15;
+						oq[j] += (__float2int_rd(amp * sn) * dp.fm_level) >> 15;
+					}
+					phA += stA; phB += stB; kq += (float) S;
+				}
+			}
+		}
+		if(am)
+		{
+			unsigned long long phM = L.phM;
+			const unsigned long long stM = dp.am_ang * S;
+			float kq = kf;
+			#pragma unroll
+			for(int j = 0; j < 4; j++)
+			{
+				if(kq > 32767.0f) kq -= 32767.0f;
+				const float amp = 32767.99998f - kq * 1.52587890625e-5f;
+				float sn, cs;
+				__sincosf((float) (int) (phM >> 32) * 1.4629180792671596e-9f, &sn, &cs);
+				const int smp = S * j >= nb ? L.amB : L.amA;
+				oi[j] += (((__float2int_rd(amp * cs) * smp) >> 15) * dp.am_level) >> 15;
+				oq[j] += (((__float2int_rd(amp * sn) * smp) >> 15) * dp.am_level) >> 15;
+				phM += stM; kq += (float) S;
+			}
+		}
+	}
+
+	if((PART & 2) && KL_HAS(SND, KL_NIC, dp.have_nicam))
+	{
+		int bi[4], bq[4];
+		if(!L.gen)
+		{
+			// pulse-shaping table (htv_tables.c): one entry per sample and channel
+			#pragma unroll
+			for(int j = 0; j < 4; j++)
+			{
+				const bool b = S * j >= L.nbs;
+				bi[j] = __ldg(dt.nicam_lut + S * j + (b ? L.niB : L.niA));
+				bq[j] = __ldg(dt.nicam_lut + S * j + (b ? L.nqB : L.nqA));
+			}
+		}
+		else nic_generic(bi, bq);   // the pulse table holds the same integer sums (htv_tables.c): the two forms agree
+		// carrier table extended past its period (htv_tables.c): cc + u never wraps
+		const htv_c16_t *ccp = dt.nicam_cc + L.cc;
+		#pragma unroll
+		for(int j = 0; j < 4; j++)
+		{
+			const short2 cc = kl_ldc16(ccp + S * j);
+			// the overlap-add ring holds at most 7 pulses of < 2^11: it never wraps an int16
+			oi[j] += (bi[j] * cc.x - bq[j] * cc.y) >> 15;
+			oq[j] += (bi[j] * cc.y + bq[j] * cc.x) >> 15;
+		}
+	}
+}
+
 // ---- mixers after the modulation (ref video.c:3466-3515): IQ swap, frequency-offset mixer --------------------------
 // Every addition before them is an int16 wrap-around addition in the reference. oi / oq stay unwrapped where only their
 // low 16 bits reach the store; the mixer, which multiplies, wraps its inputs first.
@@ -230,6 +364,43 @@ __device__ __forceinline__ void kl_mix(const htv_dparams_t &dp, const DevTables 
 				const int kk = (int) (m % 32767);
 				const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
 				const unsigned long long ph = off0 + dp.offset_ang * (unsigned long long) (x + 1);
+				float sn, cs;
+				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
+				bi = min(__float2int_rd(amp * cs), 32767); bq = min(__float2int_rd(amp * sn), 32767);   // pi >> 16 <= 32767
+			}
+			oi[j] = (vi * bi - vq * bq) >> 15;
+			oq[j] = (vi * bq + vq * bi) >> 15;
+		}
+	}
+}
+
+template<int SND, int S>
+__device__ __forceinline__ void kl_mix_lane(const htv_dparams_t &dp, const DevTables &dt, const KlLane &L, int (&oi)[4], int (&oq)[4])
+{
+	if(KL_HAS(SND, KL_SWAP, dp.swap_iq))
+	{
+		#pragma unroll
+		for(int j = 0; j < 4; j++) { const int t = oi[j]; oi[j] = oq[j]; oq[j] = t; }
+	}
+	if(KL_HAS(SND, KL_OFF, dp.have_offset))
+	{
+		#pragma unroll
+		for(int j = 0; j < 4; j++)
+		{
+			const long long m = L.m + S * j;
+			const int vi = wrap16i(oi[j]), vq = wrap16i(oq[j]);
+			int bi, bq;
+			if(m < 32767)
+			{
+				const unsigned char st = dt.offset_start[m];
+				bi = -(st & 1); bq = -((st >> 1) & 1);
+			}
+			else
+			{
+				int kk = L.kk + S * j;
+				if(kk >= 32767) kk -= 32767;
+				const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
+				const unsigned long long ph = L.offph + dp.offset_ang * (unsigned long long) (S * j);
 				float sn, cs;
 				__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);
 				bi = min(__float2int_rd(amp * cs), 32767); bq = min(__float2int_rd(amp * sn), 32767);   // pi >> 16 <= 32767
