@@ -82,7 +82,14 @@ class Frame(C.Structure):
     _fields_ = [("width", C.c_int), ("height", C.c_int), ("framebuffer", C.c_void_p), ("serial", C.c_uint64)]
 
 
+class DeviceFrame(C.Structure):
+    """htv_device_frame_t: a picture of three uint8 channels in device memory, strides in bytes"""
+    _fields_ = [("width", C.c_int), ("height", C.c_int), ("data", C.c_void_p),
+                ("stride_x", C.c_int64), ("stride_y", C.c_int64), ("stride_c", C.c_int64), ("serial", C.c_uint64)]
+
+
 _READ_VIDEO = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(Frame))
+_READ_VIDEO_DEVICE = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(DeviceFrame))
 _READ_AUDIO = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t))
 _PASSTHRU_READ = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)
 
@@ -151,6 +158,8 @@ def lib() -> C.CDLL:
     L.htv_av_close.restype = None; L.htv_av_close.argtypes = [C.POINTER(AV)]
     L.htv_av_memory_open.restype = C.c_int
     L.htv_av_memory_open.argtypes = [C.POINTER(AV), vp, sz, vp, sz, sz, C.c_int]
+    L.htv_set_video_device_source.restype = C.c_int
+    L.htv_set_video_device_source.argtypes = [vp, _READ_VIDEO_DEVICE, vp]
     L.htv_next_line.restype = C.POINTER(Line); L.htv_next_line.argtypes = [vp]
     L.htv_set_prefetch.restype = C.c_int; L.htv_set_prefetch.argtypes = [vp, C.c_int]
     L.htv_render.restype = C.c_int; L.htv_render.argtypes = [vp, C.c_int, vp, C.POINTER(sz), vp]
@@ -323,6 +332,46 @@ class Encoder:
             cb = _READ_AUDIO(read_audio)
             av.read_audio = cb
             self._keep += [cb, audio]
+
+    def set_device_source(self, frames, *, static_video: bool = False):
+        """htv_set_video_device_source over pictures in device memory: any object with __cuda_array_interface__ (a torch
+        tensor, a CuPy array, ...) of uint8, shape [n, active_lines, active_width, 3 or 4] (channels last: RGB, RGBA)
+        or [n, 3, active_lines, active_width] (channels first), any strides. Used cyclically, one picture per video
+        frame; static_video promises they never change, so each is converted once. The object is kept alive, and its
+        pictures must stay unchanged until the render call that pulled them has completed on its stream. render
+        converts them after the work queued on its stream before the call; for render_host and next_line they must be
+        complete on the device when the call is made. Replaces the video of set_source / open_memory_source (their
+        sound stays); only before the first rendered line. The render call refuses pictures of another size and memory
+        that is not on the encoder's device."""
+        cai = frames.__cuda_array_interface__
+        shape = tuple(int(v) for v in cai["shape"])
+        if cai["typestr"] != "|u1" or len(shape) != 4 or shape[0] < 1:
+            raise ValueError(f"device pictures are uint8 [n, H, W, 3|4] or [n, 3, H, W]; got {cai['typestr']} {shape}")
+        strides = cai.get("strides")
+        if strides is None:
+            strides = (shape[1] * shape[2] * shape[3], shape[2] * shape[3], shape[3], 1)
+        strides = tuple(int(v) for v in strides)
+        if shape[3] in (3, 4):
+            (n, h, w, _), (sn, sy, sx, sc) = shape, strides
+        elif shape[1] == 3:
+            (n, _, h, w), (sn, sc, sy, sx) = shape, strides
+        else:
+            raise ValueError(f"device pictures are uint8 [n, H, W, 3|4] or [n, 3, H, W]; got {shape}")
+        base = int(cai["data"][0])
+        state = {"f": 0}
+
+        def read_video(ctx, fr):
+            f = fr.contents
+            f.width, f.height = w, h
+            f.data = base + (state["f"] % n) * sn
+            f.stride_x, f.stride_y, f.stride_c = sx, sy, sc
+            f.serial = 1 if static_video else state["f"] + 1
+            state["f"] += 1
+            return HTV_OK
+        cb = _READ_VIDEO_DEVICE(read_video)
+        if self._L.htv_set_video_device_source(self._h, cb, None) != HTV_OK:
+            raise RuntimeError("htv_set_video_device_source failed (it must precede the first rendered line)")
+        self._keep += [cb, frames]
 
     def open_memory_source(self, frames: np.ndarray | None, audio: np.ndarray | None, *, audio_block: int = 0,
                            static_video: bool = False):

@@ -18,6 +18,7 @@
 #define MAX_FRAME_SLOTS 16
 #define MAX_NEW_FRAMES 7
 #define MAX_CHUNK_SECONDS 4.0
+_Static_assert(MAX_NEW_FRAMES <= HTV_INGEST_MAX, "a call's new pictures are one k_ingest list at most");
 #define PT_MAX_LINES 4096
 
 struct htv_t {
@@ -44,6 +45,8 @@ struct htv_t {
 	uint64_t cur_serial;
 	int have_serial;
 	int next_slot;
+	htv_read_video_device_t dev_read;   /* htv_set_video_device_source: used while av.read_video is NULL */
+	void *dev_ctx;
 
 	/* audio */
 	int64_t audio_have;           /* source pairs uploaded so far (absolute count) */
@@ -282,6 +285,20 @@ void htv_set_kernel_timing(htv_t *s, int on) { htv_dev_set_timing(s->dev, on); }
 float htv_last_line_kernel_ms(htv_t *s) { return(htv_dev_last_line_ms(s->dev)); }
 int htv_last_line_kernel_lines(const htv_t *s) { return(htv_dev_last_line_count(s->dev)); }
 
+int htv_set_video_device_source(htv_t *s, htv_read_video_device_t read, void *ctx)
+{
+	if(!s) return(HTV_ERROR);
+	if(s->next_line != 0)
+	{
+		fprintf(stderr, "hacktv_b200: the video source must be set before the first line is rendered\n");
+		return(HTV_ERROR);
+	}
+	s->av.read_video = NULL;
+	s->dev_read = read;
+	s->dev_ctx = ctx;
+	return(HTV_OK);
+}
+
 /* audio fetches completed up to and including audio-clock sample m (ref video.c:3273-3276) */
 static int64_t fetches_by(int64_t m, unsigned int rate)
 {
@@ -462,6 +479,14 @@ static int send_overlays(htv_t *s, long long end_line)
 	return(htv_dev_set_overlays(s->rdev, n, line, from, to, value, add));
 }
 
+/* New pictures for slots slot .. slot + n - 1: from device memory converted in place (k_ingest), from host memory one
+ * copy of n pictures that follow each other there, starting at pics[0].data */
+static int send_pictures(htv_t *s, int dev, int slot, int n, const htv_device_frame_t *pics, void *stream)
+{
+	if(dev) return(htv_dev_ingest_frames(s->rdev, slot, n, pics, stream));
+	return(htv_dev_upload_frames(s->rdev, slot, n, (const uint32_t *) pics[0].data, stream));
+}
+
 /* One device launch sequence for lines [L0, L0 + n): at most MAX_NEW_FRAMES new pictures */
 static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream)
 {
@@ -475,8 +500,8 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 	const int64_t fm = (L0 >= 2 ? L0 - 2 : 0) / s->lines, f0 = L0 / s->lines, f1 = (L0 + n - 1) / s->lines;
 	int32_t map[4096];
 	int64_t f;
-	int r, nmap = 0, run_n = 0, run_slot = 0;
-	const uint32_t *run_src = NULL;
+	int r, nmap = 0, run_n = 0, run_slot = 0, run_dev = 0;
+	htv_device_frame_t run[HTV_INGEST_MAX];       /* the pictures of the run of new ones not sent yet */
 	const size_t fpix = (size_t) rdp->active_width * rdp->active_lines;
 	void *up, *rup;
 
@@ -502,7 +527,8 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 	{
 		if(f > s->cur_frame)
 		{
-			htv_frame_t fr;
+			htv_device_frame_t pic;
+			int dev = 0, got = 0;
 			if(nnew >= MAX_NEW_FRAMES)
 			{
 				/* every free picture slot is in use by this launch: stop at this frame boundary */
@@ -515,45 +541,60 @@ static int render_chunk(htv_t *s, int *pn, int16_t *d_out, int add, void *stream
 				n = (int) (f * s->lines - L0);
 				break;
 			}
-			memset(&fr, 0, sizeof(fr));
+			memset(&pic, 0, sizeof(pic));
 			s->prev_slot = s->cur_slot;
 			s->cur_frame = f;
-			if(s->av.read_video && s->av.read_video(s->av.ctx, &fr) == HTV_OK && fr.framebuffer)
+			if(s->av.read_video)
 			{
-				if(fr.width != rdp->active_width || fr.height != rdp->active_lines)
+				htv_frame_t fr;
+				memset(&fr, 0, sizeof(fr));
+				s->dev_read = NULL;                      /* a read_video installed after a device source replaces it */
+				got = s->av.read_video(s->av.ctx, &fr) == HTV_OK && fr.framebuffer;
+				pic.width = fr.width; pic.height = fr.height; pic.data = fr.framebuffer; pic.serial = fr.serial;
+			}
+			else if(s->dev_read)
+			{
+				dev = 1;
+				got = s->dev_read(s->dev_ctx, &pic) == HTV_OK && pic.data;
+			}
+			if(got)
+			{
+				if(pic.width != rdp->active_width || pic.height != rdp->active_lines)
 				{
 					fprintf(stderr, "hacktv_b200: source frame is %dx%d, the raster needs %dx%d\n",
-						fr.width, fr.height, rdp->active_width, rdp->active_lines);
+						pic.width, pic.height, rdp->active_width, rdp->active_lines);
 					UP_FAIL(HTV_ERROR);
 				}
-				if(!s->have_serial || fr.serial != s->cur_serial || s->cur_slot < 0)
+				if(!s->have_serial || pic.serial != s->cur_serial || s->cur_slot < 0)
 				{
 					s->cur_slot = s->next_slot;
 					s->next_slot = (s->next_slot + 1) % MAX_FRAME_SLOTS;
-					/* pictures that follow each other in the caller's memory (a capture ring, htv_av_memory_open's array)
-					 * and land in consecutive slots go up as ONE copy: 2 MB copies beside the 8 MB copies coming back
-					 * keep neither PCIe direction full */
-					if(run_n > 0 && fr.framebuffer == run_src + (size_t) run_n * fpix && s->cur_slot == run_slot + run_n) run_n++;
+					/* new pictures that land in consecutive slots are sent together: from the device as one k_ingest list;
+					 * from the host when they follow each other in the caller's memory (a capture ring, htv_av_memory_open's
+					 * array), as ONE copy: 2 MB copies beside the 8 MB copies coming back keep neither PCIe direction full */
+					if(run_n > 0 && dev == run_dev && s->cur_slot == run_slot + run_n
+						&& (dev || (const uint32_t *) pic.data == (const uint32_t *) run[0].data + (size_t) run_n * fpix)) run[run_n++] = pic;
 					else
 					{
-						if(run_n > 0 && (r = htv_dev_upload_frames(s->rdev, run_slot, run_n, run_src, rup)) != HTV_OK) UP_FAIL(r);
-						run_src = fr.framebuffer; run_slot = s->cur_slot; run_n = 1;
+						if(run_n > 0 && (r = send_pictures(s, run_dev, run_slot, run_n, run, rup)) != HTV_OK) UP_FAIL(r);
+						run[0] = pic; run_slot = s->cur_slot; run_n = 1; run_dev = dev;
 					}
-					s->cur_serial = fr.serial;
+					s->cur_serial = pic.serial;
 					s->have_serial = 1;
 					nnew++;
 				}
 			}
 			else
 			{
-				if(s->av.read_video) s->av.read_video = NULL;
+				s->av.read_video = NULL;
+				s->dev_read = NULL;
 				s->cur_slot = -1;
 			}
 			if(s->vbi_read) pull_overlays(s, f);
 		}
 		map[nmap++] = s->cur_slot;
 	}
-	if(run_n > 0 && (r = htv_dev_upload_frames(s->rdev, run_slot, run_n, run_src, rup)) != HTV_OK) UP_FAIL(r);
+	if(run_n > 0 && (r = send_pictures(s, run_dev, run_slot, run_n, run, rup)) != HTV_OK) UP_FAIL(r);
 	/* sound: everything the audio clock reaches inside this run */
 	if(dp->have_fm || dp->have_am || dp->have_nicam)
 	{
@@ -628,6 +669,8 @@ static int render_any(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, in
 		fprintf(stderr, "hacktv_b200: the output buffer must be %d-byte aligned\n", align);
 		return(HTV_ERROR);
 	}
+	/* pictures from device memory are converted after whatever the caller queued on its stream before this call */
+	if(s->dev_read && !s->av.read_video && (r = htv_dev_mark_call(s->rdev, cuda_stream)) != HTV_OK) return(r);
 	cap = max_chunk_lines(s);
 	if(s->pt_read && cap > PT_MAX_LINES) cap = PT_MAX_LINES;
 	while(done < nlines)

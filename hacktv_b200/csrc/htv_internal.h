@@ -182,6 +182,13 @@ extern int htv_dev_set_overlays(htv_dev_t *d, int n, const long long *line, cons
 	const int *value, const int16_t *const *add);
 extern int htv_dev_upload_frame(htv_dev_t *d, int slot, const uint32_t *rgb, void *stream);
 extern int htv_dev_upload_frames(htv_dev_t *d, int slot, int count, const uint32_t *rgb, void *stream);
+/* pictures a launch of k_ingest takes: a call's new pictures (htv_host.c MAX_NEW_FRAMES) and one more */
+#define HTV_INGEST_MAX 8
+/* `count` device pictures into consecutive slots: k_ingest on `stream`, behind the caller's stream as
+ * htv_dev_mark_call found it; HTV_ERROR with a message for memory that is not on the encoder's device */
+extern int htv_dev_ingest_frames(htv_dev_t *d, int slot, int count, const htv_device_frame_t *frames, void *stream);
+/* the point of the caller's stream that the next ingests wait for: all work enqueued on it so far */
+extern int htv_dev_mark_call(htv_dev_t *d, void *stream);
 /* slot_of_frame[i] = slot holding frame (first_frame + i) for this launch */
 extern int htv_dev_set_frame_map(htv_dev_t *d, const int32_t *slot_of_frame, int n, int64_t first_frame, void *stream);
 /* raw audio ring <- host PCM pairs for absolute indices [j0, j0 + n) */

@@ -241,6 +241,7 @@ struct htv_dev_t {
 	cudaEvent_t ev_up, ev_chunk[2];
 	cudaStream_t pic;                 // the conversions (k_compose, k_picture), each behind its picture's copy but off the
 	cudaEvent_t ev_pic;               // upload stream, so that the next copies do not queue behind the conversions
+	cudaEvent_t ev_call;              // the caller's stream at the start of a render call that pulls device pictures
 	cudaEvent_t *ev_slot;             // [max_slots] the copy of each slot's last picture is done
 	uint8_t *comp_valid;              // [max_slots] the phases of each slot's composite rows that hold its picture (bit p)
 	int *vf_conv, vf_nconv;           // filtered store: the composite-store entries converted since the last k_vf_rows
@@ -2888,12 +2889,12 @@ static void launch_vf_rows(htv_dev_t *d, const VfConv &cv, int64_t first, int ne
 
 // An encoder's side streams and events, in the one list htv_dev_create creates and htv_dev_destroy destroys. ev0 and
 // ev1 time the last modulator launch (htv_dev_last_line_ms); every other event only orders work, without timing.
-struct DevSync { cudaStream_t *stream[5]; cudaEvent_t *timed[2]; cudaEvent_t *event[10]; };
+struct DevSync { cudaStream_t *stream[5]; cudaEvent_t *timed[2]; cudaEvent_t *event[11]; };
 static DevSync dev_sync(htv_dev_t *d)
 {
 	return(DevSync{ { &d->side, &d->side2, &d->side3, &d->up, &d->pic }, { &d->ev0, &d->ev1 },
 		{ &d->ev_nic, &d->ev_up, &d->ev_chunk[0], &d->ev_chunk[1], &d->ev_in, &d->ev_kl[0], &d->ev_kl[1], &d->ev_r2, &d->ev_audio,
-		  &d->ev_pic } });
+		  &d->ev_pic, &d->ev_call } });
 }
 
 // htv_dev_create's way out: the message, and everything allocated so far freed
@@ -3317,6 +3318,66 @@ extern "C" int htv_dev_upload_frames(htv_dev_t *d, int slot, int count, const ui
 		CK(cudaMemcpyAsync(d->d_frames + (size_t) (slot + at) * d->frame_pixels, rgb + (size_t) at * d->frame_pixels,
 			d->frame_pixels * 4 * (size_t) n, cudaMemcpyHostToDevice, (cudaStream_t) stream));
 		const int r = slots_uploaded(d, slot + at, n, (cudaStream_t) stream);
+		if(r != HTV_OK) return(r);
+	}
+	return(HTV_OK);
+}
+
+// The pictures of one k_ingest launch, by value: the kernel parameter holds them, nothing goes up before the launch
+struct IngestList { htv_device_frame_t f[HTV_INGEST_MAX]; };
+
+// A picture from device memory into a slot (htv_set_video_device_source): three strided uint8 channels to the slot's
+// R << 16 | G << 8 | B words, which every raster path reads as it reads an uploaded picture. One CTA per row blockIdx.x
+// of picture blockIdx.y, into slot slot0 + blockIdx.y; the stores are coalesced, the loads are as the strides make them
+__global__ void __launch_bounds__(256)
+k_ingest(uint32_t *frames, int width, int lines, int slot0, const __grid_constant__ IngestList list)
+{
+	const htv_device_frame_t &f = list.f[blockIdx.y];
+	const uint8_t *row = (const uint8_t *) f.data + (int64_t) blockIdx.x * f.stride_y;
+	uint32_t *out = frames + ((size_t) (slot0 + blockIdx.y) * lines + blockIdx.x) * width;
+	for(int x = threadIdx.x; x < width; x += blockDim.x)
+	{
+		const uint8_t *p = row + (int64_t) x * f.stride_x;
+		out[x] = (uint32_t) p[0] << 16 | (uint32_t) p[f.stride_c] << 8 | (uint32_t) p[2 * f.stride_c];
+	}
+}
+
+extern "C" int htv_dev_mark_call(htv_dev_t *d, void *stream)
+{
+	DevGuard guard(d->device);
+	CK(cudaEventRecord(d->ev_call, (cudaStream_t) stream));
+	return(HTV_OK);
+}
+
+// `count` pictures in device memory into `count` consecutive slots, on `stream` behind the caller's stream at the start
+// of the render call (htv_dev_mark_call). Split as htv_dev_upload_frames splits its copy: with a store, the last picture
+// is a launch of its own, so that the earlier ones are converted while it is ingested.
+extern "C" int htv_dev_ingest_frames(htv_dev_t *d, int slot, int count, const htv_device_frame_t *frames, void *stream)
+{
+	DevGuard guard(d->device);
+	if(slot < 0 || count < 1 || count > HTV_INGEST_MAX || slot + count > d->max_slots) return(HTV_ERROR);
+	for(int i = 0; i < count; i++)
+	{
+		cudaPointerAttributes pa;
+		if(cudaPointerGetAttributes(&pa, frames[i].data) != cudaSuccess) { cudaGetLastError(); pa.type = cudaMemoryTypeUnregistered; }
+		if((pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != d->device)
+		{
+			fprintf(stderr, "hacktv_b200: a device source picture must be device or managed memory on CUDA device %d\n", d->device);
+			return(HTV_ERROR);
+		}
+	}
+	const cudaStream_t st = (cudaStream_t) stream;
+	CK(cudaStreamWaitEvent(st, d->ev_call, 0));
+	const int head = d->ev_slot && count > 1 ? count - 1 : count;
+	for(int at = 0, n = head; at < count; at += n, n = count - at)
+	{
+		IngestList list;
+		memset(&list, 0, sizeof(list));
+		memcpy(list.f, frames + at, sizeof(htv_device_frame_t) * n);
+		k_ingest<<<dim3(d->dp.active_lines, n), 256, 0, st>>>(d->d_frames, d->dp.active_width, d->dp.active_lines, slot + at, list);
+		d->launches++;
+		CK(cudaGetLastError());
+		const int r = slots_uploaded(d, slot + at, n, st);
 		if(r != HTV_OK) return(r);
 	}
 	return(HTV_OK);

@@ -177,6 +177,28 @@ typedef struct {
 	htv_av_close_t close;
 } htv_av_t;
 
+/* A picture in device memory: width x height (= active_width x active_lines) pixels of three uint8 channels.
+ * R of pixel (x, y) is at data + y * stride_y + x * stride_x, G at + stride_c, B at + 2 * stride_c (bytes, signed):
+ * HWC or CHW, RGB, RGBA, BGR (negative stride_c from B's address + 2) or the encoder's own RGB32 words. */
+typedef struct {
+	int width, height;
+	const void *data;             /* device or managed memory on the encoder's device */
+	int64_t stride_x, stride_y, stride_c;
+	uint64_t serial;              /* as htv_frame_t: unchanged = the same picture, not ingested again */
+} htv_device_frame_t;
+typedef int (*htv_read_video_device_t)(void *ctx, htv_device_frame_t *frame);
+/* htv_set_video_device_source (below): a video source in device memory, pulled as read_video is: once per frame, at
+ * its first line. A return other than HTV_OK, or a NULL data, ends the source (the lines fall back to black). Each
+ * new picture is converted on the device into a picture slot (k_ingest) instead of being copied across PCIe. It
+ * replaces av->read_video (which is set to NULL; read_audio and close stay), and a read_video installed afterwards
+ * replaces it. Allowed only before the first line is rendered. The render call returns HTV_ERROR for a picture of
+ * another size, or for a `data` that is not device or managed memory of the encoder's device.
+ * Ordering: htv_render (and htv_render_add) converts a picture after all work enqueued on its cuda_stream before the
+ *   call, so a picture produced on that stream needs no synchronisation. htv_render_host and htv_next_line: the
+ *   picture must be complete on the device when `read` returns.
+ * Lifetime: in every case the picture must stay unchanged until the call that pulled it has completed on its
+ *   stream. */
+
 /* ---- parity with the reference (what "drop-in" means numerically) --------
  * Against the reference's CPU path on the same picture and sound (tests/test_gpu_*.py, tests/golden/):
  *  - bit-exact wherever the path is integer-only: raster, sync pulses, PAL / NTSC chroma, SECAM chroma (its
@@ -230,6 +252,8 @@ extern void htv_av_close(htv_av_t *av);
  * != 0 promises the pictures never change, so each is uploaded once. Pointers are borrowed. */
 extern int htv_av_memory_open(htv_av_t *av, const uint32_t *frames, size_t nframes,
 	const int16_t *audio, size_t audio_pairs, size_t audio_block, int static_video);
+/* Pictures from device memory (htv_device_frame_t above); HTV_ERROR after the first rendered line */
+extern int htv_set_video_device_source(htv_t *s, htv_read_video_device_t read, void *ctx);
 
 /* VBI overlays - the hook the reference's VBI stages (teletext, WSS, VITS, VITC, CC608; registered
  * behind the raster and SECAM stages, ref video.c:4213-4357) need from the encoder: each of them adds an
