@@ -88,9 +88,20 @@ class DeviceFrame(C.Structure):
                 ("stride_x", C.c_int64), ("stride_y", C.c_int64), ("stride_c", C.c_int64), ("serial", C.c_uint64)]
 
 
+HTV_PCM_INT16, HTV_PCM_FLOAT32 = 0, 1
+_PCM_FORMATS = {"<i2": HTV_PCM_INT16, "<f4": HTV_PCM_FLOAT32}     # __cuda_array_interface__ typestr -> format
+
+
+class DeviceAudio(C.Structure):
+    """htv_device_audio_t: a block of stereo PCM in device memory, strides in bytes"""
+    _fields_ = [("data", C.c_void_p), ("npairs", C.c_size_t), ("format", C.c_int32),
+                ("stride_pair", C.c_int64), ("stride_ch", C.c_int64)]
+
+
 _READ_VIDEO = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(Frame))
 _READ_VIDEO_DEVICE = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(DeviceFrame))
 _READ_AUDIO = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t))
+_READ_AUDIO_DEVICE = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(DeviceAudio))
 _PASSTHRU_READ = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)
 
 
@@ -160,6 +171,8 @@ def lib() -> C.CDLL:
     L.htv_av_memory_open.argtypes = [C.POINTER(AV), vp, sz, vp, sz, sz, C.c_int]
     L.htv_set_video_device_source.restype = C.c_int
     L.htv_set_video_device_source.argtypes = [vp, _READ_VIDEO_DEVICE, vp]
+    L.htv_set_audio_device_source.restype = C.c_int
+    L.htv_set_audio_device_source.argtypes = [vp, _READ_AUDIO_DEVICE, vp]
     L.htv_next_line.restype = C.POINTER(Line); L.htv_next_line.argtypes = [vp]
     L.htv_set_prefetch.restype = C.c_int; L.htv_set_prefetch.argtypes = [vp, C.c_int]
     L.htv_render.restype = C.c_int; L.htv_render.argtypes = [vp, C.c_int, vp, C.POINTER(sz), vp]
@@ -372,6 +385,46 @@ class Encoder:
         if self._L.htv_set_video_device_source(self._h, cb, None) != HTV_OK:
             raise RuntimeError("htv_set_video_device_source failed (it must precede the first rendered line)")
         self._keep += [cb, frames]
+
+    def set_device_audio(self, audio, *, audio_block: int = 0):
+        """htv_set_audio_device_source over 32 kHz stereo PCM in device memory: any object with __cuda_array_interface__
+        of int16 or float32 (converted as the header says: rint(x * 32767) clamped, NaN = 0), shape [n, 2] (pairs,
+        interleaved) or [2, n] (channels, planar), any strides. Used cyclically, audio_block pairs per pull (0 = all),
+        as set_source uses a host array. The object is kept alive, and its samples must stay unchanged until the render
+        call that took them has completed on its stream. render reads them after the work queued on its stream before
+        the call; for render_host and next_line they must be complete on the device when the call is made. Replaces
+        the sound of set_source / open_memory_source (their video stays); only before the first rendered line. The
+        render call refuses memory that is not on the encoder's device."""
+        cai = audio.__cuda_array_interface__
+        shape = tuple(int(v) for v in cai["shape"])
+        fmt = _PCM_FORMATS.get(cai["typestr"])
+        if fmt is None or len(shape) != 2 or 2 not in shape:
+            raise ValueError(f"device audio is int16 or float32 [n, 2] or [2, n]; got {cai['typestr']} {shape}")
+        size = 2 if fmt == HTV_PCM_INT16 else 4
+        strides = cai.get("strides")
+        strides = (shape[1] * size, size) if strides is None else tuple(int(v) for v in strides)
+        if shape[1] == 2:
+            (n, _), (sp, sc) = shape, strides
+        else:
+            (_, n), (sc, sp) = shape, strides
+        if n < 1:
+            raise ValueError("device audio holds no pairs")
+        base = int(cai["data"][0])
+        blk = audio_block or n
+        state = {"a": 0}
+
+        def read_audio(ctx, block):
+            at = state["a"]
+            b = block.contents
+            b.npairs = min(blk, n - at)
+            b.data = base + at * sp
+            b.format, b.stride_pair, b.stride_ch = fmt, sp, sc
+            state["a"] = (at + b.npairs) % n
+            return HTV_OK
+        cb = _READ_AUDIO_DEVICE(read_audio)
+        if self._L.htv_set_audio_device_source(self._h, cb, None) != HTV_OK:
+            raise RuntimeError("htv_set_audio_device_source failed (it must precede the first rendered line)")
+        self._keep += [cb, audio]
 
     def open_memory_source(self, frames: np.ndarray | None, audio: np.ndarray | None, *, audio_block: int = 0,
                            static_video: bool = False):

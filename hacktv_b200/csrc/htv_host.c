@@ -50,8 +50,10 @@ struct htv_t {
 
 	/* audio */
 	int64_t audio_have;           /* source pairs uploaded so far (absolute count) */
-	const int16_t *pend_pcm;      /* rest of a source block larger than one ring piece: uploaded before the next read */
-	size_t pend_n;
+	htv_device_audio_t pend;      /* rest of a source block larger than one ring piece: sent before the next read */
+	int pend_dev;                 /* ... and whether it is in device memory */
+	htv_read_audio_device_t adev_read;  /* htv_set_audio_device_source: used while av.read_audio is NULL */
+	void *adev_ctx;
 	int16_t *zeros;
 
 	/* VBI overlays pulled from the source, kept until their line has been rendered */
@@ -299,51 +301,91 @@ int htv_set_video_device_source(htv_t *s, htv_read_video_device_t read, void *ct
 	return(HTV_OK);
 }
 
+int htv_set_audio_device_source(htv_t *s, htv_read_audio_device_t read, void *ctx)
+{
+	if(!s) return(HTV_ERROR);
+	if(s->next_line != 0)
+	{
+		fprintf(stderr, "hacktv_b200: the sound source must be set before the first line is rendered\n");
+		return(HTV_ERROR);
+	}
+	s->av.read_audio = NULL;
+	s->adev_read = read;
+	s->adev_ctx = ctx;
+	return(HTV_OK);
+}
+
 /* audio fetches completed up to and including audio-clock sample m (ref video.c:3273-3276) */
 static int64_t fetches_by(int64_t m, unsigned int rate)
 {
 	return((int64_t) (((unsigned long long) (m + 1) * HTV_AUDIO_RATE) / rate));
 }
 
+/* host PCM (read_audio's interleaved int16 pairs) described as a block */
+static htv_device_audio_t host_block(const int16_t *pcm, size_t npairs)
+{
+	htv_device_audio_t b;
+	b.data = pcm; b.npairs = npairs; b.format = HTV_PCM_INT16;
+	b.stride_pair = 2 * sizeof(int16_t); b.stride_ch = sizeof(int16_t);
+	return(b);
+}
+
 /* Make source audio available on the device up to pair index `need` (exclusive). A source may hand
  * over blocks of any size (ref video.c:3280): one larger than a quarter of the device ring goes up in
- * ring-sized pieces, the remainder kept for the next calls - nothing is dropped. */
+ * ring-sized pieces, the remainder kept for the next calls - nothing is dropped. Host blocks are copied
+ * up, device blocks (htv_set_audio_device_source) converted into the ring on the device. */
 static int pull_audio(htv_t *s, int64_t need, void *stream)
 {
 	const size_t piece = htv_dev_audio_ring_pairs() / 4;
 	while(s->audio_have < need)
 	{
-		const int16_t *pcm = s->pend_pcm;
-		size_t n = s->pend_n;
-		int r = HTV_OK;
+		htv_device_audio_t b = s->pend;
+		int dev = s->pend_dev, r;
 
-		if(!n)
+		if(!b.npairs)
 		{
-			pcm = NULL;
+			memset(&b, 0, sizeof(b));
+			dev = 0;
 			if(s->av.read_audio)
 			{
-				r = s->av.read_audio(s->av.ctx, &pcm, &n);
-				if(r != HTV_OK) { s->av.read_audio = NULL; pcm = NULL; n = 0; }
+				const int16_t *pcm = NULL;
+				size_t n = 0;
+				s->adev_read = NULL;                     /* a read_audio installed after a device source replaces it */
+				if(s->av.read_audio(s->av.ctx, &pcm, &n) != HTV_OK) { s->av.read_audio = NULL; pcm = NULL; n = 0; }
+				b = host_block(pcm, n);
 			}
-			if(!pcm || n == 0)
+			else if(s->adev_read)
+			{
+				/* a device source ends at its first empty block */
+				if(s->adev_read(s->adev_ctx, &b) == HTV_OK && b.data && b.npairs) dev = 1;
+				else { s->adev_read = NULL; b.data = NULL; }
+			}
+			if(!b.data || b.npairs == 0)
 			{
 				/* no audio from the source: silence (ref video.c:3298-3303) */
-				pcm = s->zeros;
-				n = (size_t) (need - s->audio_have);
-				if(n > 65536) n = 65536;
+				size_t n = (size_t) (need - s->audio_have);
+				b = host_block(s->zeros, n > 65536 ? 65536 : n);
 			}
 		}
-		s->pend_pcm = NULL; s->pend_n = 0;
-		if(n > piece)
+		s->pend.npairs = 0;
+		if(b.npairs > piece)
 		{
 			/* only what this render call needs now (at most a piece): the device ring holds about 32 s */
 			size_t take = (size_t) (need - s->audio_have);
 			if(take > piece) take = piece;
-			if(take < n) { s->pend_pcm = pcm + take * 2; s->pend_n = n - take; n = take; }
+			if(take < b.npairs)
+			{
+				s->pend = b;
+				s->pend.data = (const char *) b.data + (int64_t) take * b.stride_pair;
+				s->pend.npairs = b.npairs - take;
+				s->pend_dev = dev;
+				b.npairs = take;
+			}
 		}
-		r = htv_dev_upload_audio(s->dev, s->audio_have, pcm, n, stream);
+		r = dev ? htv_dev_ingest_audio(s->dev, s->audio_have, &b, stream)
+			: htv_dev_upload_audio(s->dev, s->audio_have, (const int16_t *) b.data, b.npairs, stream);
 		if(r != HTV_OK) return(r);
-		s->audio_have += n;
+		s->audio_have += (int64_t) b.npairs;
 	}
 	return(HTV_OK);
 }
@@ -669,8 +711,10 @@ static int render_any(htv_t *s, int nlines, int16_t *d_out, size_t *nsamples, in
 		fprintf(stderr, "hacktv_b200: the output buffer must be %d-byte aligned\n", align);
 		return(HTV_ERROR);
 	}
-	/* pictures from device memory are converted after whatever the caller queued on its stream before this call */
+	/* pictures and sound from device memory are read after whatever the caller queued on its stream before this call;
+	 * the pictures go into the raster context, the sound into the modulating one (the same one without --pixelrate) */
 	if(s->dev_read && !s->av.read_video && (r = htv_dev_mark_call(s->rdev, cuda_stream)) != HTV_OK) return(r);
+	if(s->adev_read && !s->av.read_audio && (r = htv_dev_mark_call(s->dev, cuda_stream)) != HTV_OK) return(r);
 	cap = max_chunk_lines(s);
 	if(s->pt_read && cap > PT_MAX_LINES) cap = PT_MAX_LINES;
 	while(done < nlines)

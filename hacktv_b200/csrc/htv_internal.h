@@ -187,12 +187,16 @@ extern int htv_dev_upload_frames(htv_dev_t *d, int slot, int count, const uint32
 /* `count` device pictures into consecutive slots: k_ingest on `stream`, behind the caller's stream as
  * htv_dev_mark_call found it; HTV_ERROR with a message for memory that is not on the encoder's device */
 extern int htv_dev_ingest_frames(htv_dev_t *d, int slot, int count, const htv_device_frame_t *frames, void *stream);
-/* the point of the caller's stream that the next ingests wait for: all work enqueued on it so far */
+/* the point of the caller's stream that the next ingests (pictures and sound) wait for: all work enqueued on it so far */
 extern int htv_dev_mark_call(htv_dev_t *d, void *stream);
 /* slot_of_frame[i] = slot holding frame (first_frame + i) for this launch */
 extern int htv_dev_set_frame_map(htv_dev_t *d, const int32_t *slot_of_frame, int n, int64_t first_frame, void *stream);
 /* raw audio ring <- host PCM pairs for absolute indices [j0, j0 + n) */
 extern int htv_dev_upload_audio(htv_dev_t *d, int64_t j0, const int16_t *pcm, size_t npairs, void *stream);
+/* raw audio ring <- a block of device PCM for absolute indices [j0, j0 + block->npairs): k_pcm_ingest on `stream`,
+ * behind the caller's stream as htv_dev_mark_call found it; HTV_ERROR with a message for an unknown format, a
+ * misaligned view, or memory that is not on the encoder's device */
+extern int htv_dev_ingest_audio(htv_dev_t *d, int64_t j0, const htv_device_audio_t *block, void *stream);
 /* audio-rate pre-pass for the absolute audio-clock sample range [m0, m1) */
 extern int htv_dev_audio_prepass(htv_dev_t *d, int64_t m0, int64_t m1, void *stream);
 /* the line kernel(s): render lines [line0, line0 + nlines) to d_out (device); r is NULL, or with --pixelrate the raster

@@ -241,7 +241,7 @@ struct htv_dev_t {
 	cudaEvent_t ev_up, ev_chunk[2];
 	cudaStream_t pic;                 // the conversions (k_compose, k_picture), each behind its picture's copy but off the
 	cudaEvent_t ev_pic;               // upload stream, so that the next copies do not queue behind the conversions
-	cudaEvent_t ev_call;              // the caller's stream at the start of a render call that pulls device pictures
+	cudaEvent_t ev_call;              // the caller's stream at the start of a render call that pulls device pictures or sound
 	cudaEvent_t *ev_slot;             // [max_slots] the copy of each slot's last picture is done
 	uint8_t *comp_valid;              // [max_slots] the phases of each slot's composite rows that hold its picture (bit p)
 	int *vf_conv, vf_nconv;           // filtered store: the composite-store entries converted since the last k_vf_rows
@@ -3457,6 +3457,69 @@ extern "C" int htv_dev_upload_audio(htv_dev_t *d, int64_t j0, const int16_t *pcm
 		CK(cudaMemcpyAsync(d->d_pcm + at * 2, pcm, n * 4, cudaMemcpyHostToDevice, (cudaStream_t) stream));
 		pcm += n * 2; j0 += n; npairs -= n;
 	}
+	return(HTV_OK);
+}
+
+// One sample of a device PCM block as the int16 the ring holds (the header's rule for HTV_PCM_FLOAT32: the product
+// in float32, rounded to nearest even, clamped; NaN is 0)
+__device__ __forceinline__ short pcm_sample(const char *p, int format)
+{
+	if(format == HTV_PCM_INT16) return(*(const short *) p);
+	const float x = __fmul_rn(*(const float *) p, 32767.0f);
+	if(x != x) return(0);
+	return((short) fminf(fmaxf(rintf(x), -32768.0f), 32767.0f));
+}
+
+// A block of stereo PCM from device memory into the sound ring (htv_set_audio_device_source): pair i of the block to
+// ring pair (j0 + i) & (RA - 1), wrapping, as the int16 pair the host path copies up. One thread per pair: the stores
+// are coalesced 32-bit words, the loads are as the strides make them
+__global__ void __launch_bounds__(256)
+k_pcm_ingest(short2 *ring, int64_t j0, const __grid_constant__ htv_device_audio_t b)
+{
+	const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
+	if(i >= (int64_t) b.npairs) return;
+	const char *p = (const char *) b.data + i * b.stride_pair;
+	ring[(j0 + i) & (RA - 1)] = make_short2(pcm_sample(p, b.format), pcm_sample(p + b.stride_ch, b.format));
+}
+
+// A device PCM block into ring pairs [j0, j0 + npairs), queued where htv_dev_upload_audio queues its copy: on the
+// upload stream, between htv_dev_uploads_begin and htv_dev_uploads_end. The events that order it:
+//  - ev_call (waited for here): the block is read after all the work the caller queued on its stream before the render
+//    call, so a block written there needs no synchronise;
+//  - ev_chunk (htv_dev_uploads_begin): the upload stream runs behind the kernels of the launch sequence before last.
+//    The pairs written here lie past everything the previous sequence's pre-pass and line kernel still read (the ring
+//    holds about 32 s, a sequence at most 4 s and a piece 8 s), as with the copy;
+//  - ev_up (recorded behind the ingest at htv_dev_uploads_end): the pre-pass chains on the side streams (which run
+//    ahead, beside the previous call's line kernel) and the caller's stream wait for it, so nothing reads the new
+//    pairs before they are written.
+extern "C" int htv_dev_ingest_audio(htv_dev_t *d, int64_t j0, const htv_device_audio_t *b, void *stream)
+{
+	DevGuard guard(d->device);
+	const int64_t size = b->format == HTV_PCM_INT16 ? 2 : b->format == HTV_PCM_FLOAT32 ? 4 : 0;
+	if(!size)
+	{
+		fprintf(stderr, "hacktv_b200: unknown device PCM format %d (HTV_PCM_INT16, HTV_PCM_FLOAT32)\n", (int) b->format);
+		return(HTV_ERROR);
+	}
+	if(b->npairs == 0) return(HTV_OK);
+	if(b->npairs > RA) return(HTV_ERROR);
+	if(((int64_t) (uintptr_t) b->data | b->stride_pair | b->stride_ch) & (size - 1))
+	{
+		fprintf(stderr, "hacktv_b200: a device PCM block's address and strides must be multiples of its %d-byte samples\n", (int) size);
+		return(HTV_ERROR);
+	}
+	cudaPointerAttributes pa;
+	if(cudaPointerGetAttributes(&pa, b->data) != cudaSuccess) { cudaGetLastError(); pa.type = cudaMemoryTypeUnregistered; }
+	if((pa.type != cudaMemoryTypeDevice && pa.type != cudaMemoryTypeManaged) || pa.device != d->device)
+	{
+		fprintf(stderr, "hacktv_b200: a device source PCM block must be device or managed memory on CUDA device %d\n", d->device);
+		return(HTV_ERROR);
+	}
+	const cudaStream_t st = (cudaStream_t) stream;
+	CK(cudaStreamWaitEvent(st, d->ev_call, 0));
+	k_pcm_ingest<<<(unsigned) ((b->npairs + 255) / 256), 256, 0, st>>>((short2 *) d->d_pcm, j0, *b);
+	d->launches++;
+	CK(cudaGetLastError());
 	return(HTV_OK);
 }
 

@@ -199,6 +199,38 @@ typedef int (*htv_read_video_device_t)(void *ctx, htv_device_frame_t *frame);
  * Lifetime: in every case the picture must stay unchanged until the call that pulled it has completed on its
  *   stream. */
 
+/* A block of 32 kHz stereo PCM in device memory: npairs pairs (L, R). L of pair j is at data + j * stride_pair,
+ * R at + stride_ch (bytes, signed): interleaved [n][2] (stride_pair = 2 * size, stride_ch = size), planar [2][n]
+ * (stride_pair = size, stride_ch = n * size), R before L (negative stride_ch from L's address), every k-th pair of
+ * a larger buffer. `data` and both strides are multiples of the sample size (2 or 4 bytes).
+ *   HTV_PCM_INT16: the values go into the sound ring as they are, as from read_audio.
+ *   HTV_PCM_FLOAT32: this library's own extension, the reference takes int16 only. Each value x becomes
+ *     (int16) clamp(rint(x * 32767.0f), -32768, 32767): the product in float32, rounded to nearest with ties to
+ *     even, then clamped (so 1.0 is 32767, -1.0 is -32767, beyond +-1 saturates); NaN becomes 0. */
+#define HTV_PCM_INT16   0
+#define HTV_PCM_FLOAT32 1
+typedef struct {
+	const void *data;             /* L of pair 0; device or managed memory on the encoder's device */
+	size_t npairs;                /* stereo pairs in this block, 32 kHz, any count >= 0 */
+	int32_t format;               /* HTV_PCM_INT16 | HTV_PCM_FLOAT32 */
+	int64_t stride_pair;          /* bytes from pair j to pair j + 1 (signed) */
+	int64_t stride_ch;            /* bytes from L to R of a pair (signed) */
+} htv_device_audio_t;
+typedef int (*htv_read_audio_device_t)(void *ctx, htv_device_audio_t *block);
+/* htv_set_audio_device_source (below): a sound source in device memory, pulled whenever read_audio would be, with
+ * blocks of any size: one larger than a quarter of the device ring is taken in pieces, the rest kept for the next
+ * calls, and nothing is dropped. A return other than HTV_OK, a NULL data or npairs == 0 ends the source (silence
+ * follows, as when read_audio ends). Each block is converted on the device into the sound ring (k_pcm_ingest)
+ * instead of being copied across PCIe. It replaces av->read_audio (which is set to NULL; read_video, a device
+ * picture source and close stay), and a read_audio installed afterwards replaces it. Allowed only before the first
+ * line is rendered. The render call returns HTV_ERROR for an unknown format, for a `data` or stride that is not a
+ * multiple of the sample size, or for a `data` that is not device or managed memory of the encoder's device.
+ * Ordering: htv_render (and htv_render_add) reads a block after all work enqueued on its cuda_stream before the
+ *   call, so a block produced on that stream needs no synchronisation. htv_render_host and htv_next_line: the
+ *   block must be complete on the device when `read` returns.
+ * Lifetime: in every case the block must stay unchanged until the call that pulled it has completed on its
+ *   stream; a block taken in pieces, until the call that takes its last pair has completed. */
+
 /* ---- parity with the reference (what "drop-in" means numerically) --------
  * Against the reference's CPU path on the same picture and sound (tests/test_gpu_*.py, tests/golden/):
  *  - bit-exact wherever the path is integer-only: raster, sync pulses, PAL / NTSC chroma, SECAM chroma (its
@@ -254,6 +286,8 @@ extern int htv_av_memory_open(htv_av_t *av, const uint32_t *frames, size_t nfram
 	const int16_t *audio, size_t audio_pairs, size_t audio_block, int static_video);
 /* Pictures from device memory (htv_device_frame_t above); HTV_ERROR after the first rendered line */
 extern int htv_set_video_device_source(htv_t *s, htv_read_video_device_t read, void *ctx);
+/* Sound from device memory (htv_device_audio_t above); HTV_ERROR after the first rendered line */
+extern int htv_set_audio_device_source(htv_t *s, htv_read_audio_device_t read, void *ctx);
 
 /* VBI overlays - the hook the reference's VBI stages (teletext, WSS, VITS, VITC, CC608; registered
  * behind the raster and SECAM stages, ref video.c:4213-4357) need from the encoder: each of them adds an
