@@ -143,6 +143,16 @@ int htv_init_on(htv_t **out, int device, unsigned int sample_rate, unsigned int 
 			return(HTV_ERROR);
 		}
 		s->rtab->raster_only = 1;
+		/* the raster context's kernels are planned first, so that a pixel-rate line they cannot hold is refused
+		 * before anything is allocated or launched on the device */
+		if(htv_dev_plan_name(s->rtab, s->rtab->dp.sample_type, err, sizeof(err)) != HTV_OK)
+		{
+			fprintf(stderr, "hacktv_b200: cannot initialise the CUDA encoder: %s\n", err);
+			htv_tables_free(s->rtab);
+			htv_tables_free(s->tab);
+			free(s);
+			return(HTV_ERROR);
+		}
 	}
 
 	/* No GPU, no encoder: there is deliberately no CPU fallback */

@@ -2684,12 +2684,14 @@ static int plan_kernels(const struct htv_tables_t *t, const DevSwitches &sw, int
 	p->line_threads = ((W + 3) / 4 + 31) & ~31;
 	if(p->line_threads < 64) p->line_threads = 64;
 	p->kl_threads = 32 * T;
-	if(p->line_threads > 384) { snprintf(err, errlen, "line width %d exceeds the kernels' 1536-sample limit", W); return(HTV_ERROR); }
+	// with --pixelrate the raster runs in a context of its own, at the pixel rate: its messages name that line
+	const char *whose = t->raster_only ? "the pixel-rate raster's " : "";
+	if(p->line_threads > 384) { snprintf(err, errlen, "%sline width %d exceeds the kernels' 1536-sample limit", whose, W); return(HTV_ERROR); }
 	// The lower limit: k_line's rows carry 32 samples of each neighbouring line (KL_LEAD halos), and the split modulators
 	// stage 32 samples of the line before (EXT), so a line shorter than that would take them from two lines back. FM
 	// video's k_fmv_base stages FOFF = 40 samples of the line before from the composite stream, which starts one line
 	// early: a shorter line would read in front of it.
-	if(W < 32) { snprintf(err, errlen, "line width %d is below the kernels' 32-sample limit", W); return(HTV_ERROR); }
+	if(W < 32) { snprintf(err, errlen, "%sline width %d is below the kernels' 32-sample limit", whose, W); return(HTV_ERROR); }
 	if(dp.have_fmv && W < FOFF)
 	{
 		snprintf(err, errlen, "line width %d is below FM video's %d-sample limit", W, FOFF);

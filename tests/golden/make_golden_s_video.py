@@ -46,6 +46,23 @@ CASES = [
     ("pal", 16000000, 1300, False, ["--offset", "2000000"], "test"),
     ("pal", 16000000, 1300, True, [], "programme"),
     ("secam", 16000000, 1300, True, [], "programme"),
+    # below 10 Msps: every row of tests/test_gpu_zz_low_rate_paths.py S_VIDEO
+    ("pal", 1500000, 1300, False, [], "test"),                  # a single-warp CTA
+    ("pal", 2000000, 1300, True, [], "test"),
+    ("pal", 4000000, 1300, True, [], "test"),
+    ("pal", 6750000, 1300, True, [], "test"),
+    ("pal", 7000000, 1300, True, [], "test"),                   # chroma taps sum to 32770
+    ("pal", 8000000, 1300, True, [], "test"),
+    ("ntsc", 2000000, 1100, False, [], "test"),                 # no composite store, a single-warp CTA
+    ("ntsc", 2250000, 1100, False, [], "test"),
+    ("ntsc", 4500000, 1100, True, [], "test"),
+    ("ntsc", 7000000, 1100, True, [], "test"),                  # no composite store, chroma taps sum to 32770
+    ("pal60", 6750000, 1100, True, [], "test"),
+    ("525pal", 4500000, 1100, False, [], "test"),
+    ("secam", 2000000, 1300, False, [], "test"),
+    ("secam", 4000000, 1300, False, [], "test"),
+    ("secam", 6000000, 1300, True, [], "test"),
+    ("secam", 10000000, 1300, True, [], "test"),
 ]
 
 

@@ -1,7 +1,9 @@
 """The encoder below 10 Msps, on the device, against the oracle: every kernel form that only this band reaches.
 
 Below 10 Msps the chroma low-pass has 7, 5, 3 and finally 1 tap, and the kernel selection changes with it:
-  - k_picture's low-pass (chroma_lp4 / chroma_fir4<7|5|3>) feeds k_line, and at 7 Msps the taps sum to 32770 (CSAT);
+  - k_compose's low-pass (chroma_lp4 / chroma_fir4<7|5|3>) fills the composite store k_line reads: every colour row
+    here has P = 4 (PAL) or P = 2 (NTSC at multiples of 2.25 MHz), and at 7 Msps the taps sum to 32770 (CSAT). The
+    encoders without a composite store (P = 0), where k_picture's low-pass feeds k_line, are test_gpu_zz_low_rate_paths.py's;
   - at W <= 128 k_line's CTA is a single warp, whose lanes fill both halos of a row, and W = 96 is one partial tile;
   - at 1 tap (1.25 Msps and below for PAL and NTSC) the split modulators run behind k_raster with chroma_fir4<1>:
     k_mod_tma (4 | W), k_mod_mma (pitched planes with the video filter), k_mod (NTSC W = 79);
@@ -114,7 +116,7 @@ COLOUR_KLINE = [c for c in MATRIX if c[4].startswith("k_line") and not c[2].get(
 
 @pytest.mark.parametrize("mode,rate,kw,W,kernel", COLOUR_KLINE, ids=[case_id(c) for c in COLOUR_KLINE])
 def test_low_rate_random_pictures(built, mode, rate, kw, W, kernel):
-    """A new random picture every frame, bit-exact without sound: k_picture's 3-, 5- and 7-tap low-pass over full-range
+    """A new random picture every frame, bit-exact without sound: k_compose's 3-, 5- and 7-tap low-pass over full-range
     U and V."""
     H = built
     quiet = H.mode_config(mode, **dict(kw, noaudio=True))

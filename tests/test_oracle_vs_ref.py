@@ -94,12 +94,25 @@ def _low_rate_cases():
     return out
 
 
+def _low_rate_path_cases():
+    """Every PS row of test_gpu_zz_low_rate_paths.py (k_line without a composite store below 10 Msps), with the mode's
+    sound and the lines it renders."""
+    from test_gpu_zz_low_rate_paths import PS
+    out = []
+    for mode, rate, kw, *_ in PS:
+        case = (mode, rate, 290 if mode in ("m", "ntsc", "pal60", "pal60-i") else 340, bool(kw.get("vfilter")), ())
+        if case not in CASES and case not in out:
+            out.append(case)
+    return out
+
+
 CASES += _line_width_cases()
 CASES += _mode_matrix_cases()
 CASES += _low_rate_cases()
 # SECAM with the video filter below 5 Msps: the filter's taps ahead reach the next line's burst window (the device
 # refuses these; the oracle restates them)
 CASES += [("l", 4000000, 340, True, ()), ("l", 2000000, 340, True, ())]
+CASES += _low_rate_path_cases()
 
 
 def ref_key(mode, rate, lines, *, skip=0, vfilter=False, extra=(), source="test", rawheap=False):
@@ -413,7 +426,20 @@ def _pixelrate_matrix_cases():
     return out
 
 
+def _low_pixelrate_cases():
+    """Every --pixelrate row of test_gpu_zz_low_rate_paths.py, with the mode's sound and the lines it renders, and PAL at
+    2 Msps from 484 375 Hz: a 31-sample raster, which the oracle restates and the device refuses."""
+    from test_gpu_zz_low_rate_paths import PIXELRATE
+    out = []
+    for mode, rate, prate, kw, *_ in PIXELRATE:
+        case = (mode, rate, prate, 290 if mode in ("m", "ntsc") else 340, bool(kw.get("vfilter")), ())
+        if case not in PIXELRATE_CASES and case not in out:
+            out.append(case)
+    return out + [("pal", 2000000, 484375, 340, False, ())]
+
+
 PIXELRATE_CASES += _pixelrate_matrix_cases()
+PIXELRATE_CASES += _low_pixelrate_cases()
 
 
 @pytest.mark.parametrize("mode,rate,prate,nlines,filt,extra", PIXELRATE_CASES)
