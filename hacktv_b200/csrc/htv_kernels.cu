@@ -1854,6 +1854,15 @@ __global__ void __launch_bounds__(256) k_overlay_secam(const __grid_constant__ h
 
 #include "htv_sound.cuh"
 
+// One sample of a store to another sample type than int16 (htv_sample_type.h): the channel combiner's int16 sum with
+// wrap-around - `acc` is int16 in the output layout, never `out` itself (htv_render_add refuses other types) - then the
+// conversion. The int16 stores stay per kernel family: they move their samples packed.
+__device__ __forceinline__ void st_put_sum(int16_t *out, const int16_t *acc, size_t s, int st, bool cpx, int vi, int vq)
+{
+	if(cpx) htv_st_put2(out, s, st, wrap16i(vi + (acc ? acc[2 * s] : 0)), wrap16i(vq + (acc ? acc[2 * s + 1] : 0)));
+	else htv_st_put(out, s, st, wrap16i(vi + (acc ? acc[s] : 0)));
+}
+
 // Mixers after the modulation (htv_sound.cuh), the channel combiner and the store of 4 consecutive samples.
 // TY: the output has another sample type than int16 (dp.sample_type, htv_sample_type.h). The kernels that share this store
 // take it as a template argument, so that their int16 instantiations compile as if the conversion did not exist.
@@ -1870,15 +1879,11 @@ __device__ __forceinline__ void mod_store(const htv_dparams_t &dp, const DevTabl
 	const size_t lbase = (size_t) row * (size_t) W;
 	if constexpr(TY)
 	{
-		// another sample type: the int16 sum, then the conversion, one sample at a time; `acc` is int16 in the output
-		// layout, never `out` itself (htv_render_add refuses other types)
+		// another sample type: one sample at a time
 		#pragma unroll
 		for(int k = 0; k < SPT; k++)
 		{
-			if(x0 + k >= W) continue;
-			const size_t s = lbase + x0 + k;
-			if(dp.complex_out) htv_st_put2(out, s, dp.sample_type, wrap16i(oi[k] + (acc ? acc[2 * s] : 0)), wrap16i(oq[k] + (acc ? acc[2 * s + 1] : 0)));
-			else htv_st_put(out, s, dp.sample_type, wrap16i(oi[k] + (acc ? acc[s] : 0)));
+			if(x0 + k < W) st_put_sum(out, acc, lbase + x0 + k, dp.sample_type, dp.complex_out, oi[k], oq[k]);
 		}
 		return;
 	}
@@ -2031,17 +2036,8 @@ k_fmv_base(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const L
 	__shared__ unsigned long long red[12];
 	const int tid = threadIdx.x;
 
-	{
-		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
-		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
-	}
-	if(dp.have_nicam)
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
-		int4 *dst = reinterpret_cast<int4 *>(ntp);
-		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
-	}
+	kl_la_load(&la, lap + blockIdx.x);
+	if(dp.have_nicam) kl_tpad_load(dp, dt, ntp);
 	{
 		// the launch's composite stream starts one line early: row b begins at (b + 1) * W - or at
 		// b * W when row 0 is the pipeline's fill line (`pre`), whose history is zero
@@ -2131,11 +2127,7 @@ k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	__shared__ LineA2 la;
 	__shared__ unsigned long long wsum[12];
 	const int W = dp.W, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-	{
-		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
-		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
-	}
+	kl_la_load(&la, lap + blockIdx.x);
 	const int x0 = tid * SPT;
 	unsigned long long p[SPT];
 	unsigned long long run = 0;
@@ -2169,13 +2161,12 @@ k_fmv_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	for(int k = 0; k < SPT; k++, kk++)
 	{
 		if(kk >= 32767) kk -= 32767;
-		// amplitude of the Q31 phasor kk+1 multiplications after a renormalisation (as the sound carriers)
-		const float amp = 32767.99998f - (float) (kk + 1) * 1.52587890625e-5f;
-		const unsigned long long ph = before + p[k];
+		// the Q31 phasor kk+1 multiplications after a renormalisation (as the sound carriers)
+		const float amp = kl_amp((float) (kk + 1));
 		float sn, cs;
-		__sincosf((float) (int) (ph >> 32) * 1.4629180792671596e-9f, &sn, &cs);       // pi / 2^31
-		oi[k] = (min((int) floorf(amp * cs), 32767) * dp.fmv_level) >> 15;    // pi >> 16 <= 32767
-		oq[k] = (min((int) floorf(amp * sn), 32767) * dp.fmv_level) >> 15;
+		kl_sincos(before + p[k], sn, cs);
+		oi[k] = (min(__float2int_rd(amp * cs), 32767) * dp.fmv_level) >> 15;    // pi >> 16 <= 32767
+		oq[k] = (min(__float2int_rd(amp * sn), 32767) * dp.fmv_level) >> 15;
 	}
 	mod_store<TY>(dp, dt, &la, x0, row, oi, oq, out, row < acc_rows ? acc : NULL);
 }
@@ -2194,18 +2185,8 @@ k_mod(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineA2
 	__shared__ LineA2 la;
 	const int tid = threadIdx.x;
 
-	{
-		const int4 *sa = reinterpret_cast<const int4 *>(lap + blockIdx.x);
-		int4 *da = reinterpret_cast<int4 *>(&la);
-		for(int i = tid; i < (int) (sizeof(LineA2) / 16); i += blockDim.x) da[i] = __ldg(sa + i);
-	}
-	if(dp.have_nicam)
-	{
-		// the zero-padded pulse table (8 zeros, the pulse, zeros) is prepared on the host
-		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
-		int4 *dst = reinterpret_cast<int4 *>(ntp);
-		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
-	}
+	kl_la_load(&la, lap + blockIdx.x);
+	if(dp.have_nicam) kl_tpad_load(dp, dt, ntp);
 	{
 		// the launch's composite stream starts one line early: this line begins at (b + 1) * W
 		const int16_t *cs = comp + ((size_t) blockIdx.x + 1) * W;
@@ -2283,12 +2264,7 @@ k_mod_tma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	const int tid = threadIdx.x;
 	const unsigned bytes = (unsigned) (NW * sizeof(int) + sizeof(LineA2));
 
-	if(dp.have_nicam)
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
-		int4 *dst = reinterpret_cast<int4 *>(ntp);
-		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
-	}
+	if(dp.have_nicam) kl_tpad_load(dp, dt, ntp);
 	if(tid == 0)
 	{
 		asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(&bar[0])));
@@ -2363,12 +2339,7 @@ k_mod_mma(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const Li
 	const unsigned bytes = (unsigned) (2 * WB + sizeof(LineA2));
 	const bool hasq = dp.vf_type == 3;
 
-	if(dp.have_nicam)
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
-		int4 *dst = reinterpret_cast<int4 *>(ntp);
-		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
-	}
+	if(dp.have_nicam) kl_tpad_load(dp, dt, ntp);
 	for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
 	// the bytes behind the window are multiplied by zero taps only; the TMA never writes them
 	// (contiguous layout; a pitched row arrives whole)

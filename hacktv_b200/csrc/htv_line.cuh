@@ -98,12 +98,7 @@ __device__ __forceinline__ void kl_post_store(const htv_dparams_t &dp, const Dev
 		#pragma unroll
 		for(int j = 0; j < 4; j++)
 		{
-			if(FULL || xb + 8 * j < W)
-			{
-				const size_t s = lbase + xb + 8 * j;
-				if(cpx) htv_st_put2(out, s, st, wrap16i(oi[j] + (acc ? acc[2 * s] : 0)), wrap16i(oq[j] + (acc ? acc[2 * s + 1] : 0)));
-				else htv_st_put(out, s, st, wrap16i(oi[j] + (acc ? acc[s] : 0)));
-			}
+			if(FULL || xb + 8 * j < W) st_put_sum(out, acc, lbase + xb + 8 * j, st, cpx, oi[j], oq[j]);
 		}
 		return;
 	}
@@ -281,9 +276,7 @@ __device__ __forceinline__ void kl_nic_generic_feed(const htv_dparams_t &dp, con
 			const unsigned d = (rx + cnd * F) / D;                      // samples since symbol sx - cnd started
 			if((long long) d > m + 8 * j) break;                        // before the stream start
 			const int sy = (int) (__ldg(dt.nic_rec + ((sx - cnd) & (RS - 1))) >> 18) & 3;
-			const int r = ntp[d + NIC_TPAD];                            // the table is zero outside the pulse
-			bi[j] += (sy & 1) ? r : -r;
-			bq[j] += (sy & 2) ? r : -r;
+			kl_nic_add(sy, ntp[d + NIC_TPAD], bi[j], bq[j]);            // the table is zero outside the pulse
 		}
 	}
 }
@@ -368,12 +361,7 @@ k_line(const __grid_constant__ htv_dparams_t dp, const DevTables dt, const LineR
 	// ---- one-time set-up -------------------------------------------------------
 	if(RING) for(int i = tid; i < MF_ATAB_WORDS / 4; i += blockDim.x) atab[i] = __ldg(reinterpret_cast<const uint4 *>(dt.mma_atab) + i);
 	if(RING) for(int i = tid; i < 8 * RB / 4; i += blockDim.x) reinterpret_cast<unsigned *>(rows)[i] = 0;
-	if(KL_HAS(SND, KL_NIC, dp.have_nicam))
-	{
-		const int4 *src = reinterpret_cast<const int4 *>(dt.nicam_tpad);
-		int4 *dst = reinterpret_cast<int4 *>(ntp);
-		for(int i = tid; i < (dp.nicam_tpad_len + 7) / 8; i += blockDim.x) dst[i] = __ldg(src + i);
-	}
+	if(KL_HAS(SND, KL_NIC, dp.have_nicam)) kl_tpad_load(dp, dt, ntp);
 	if(!SRC && !FS && tid < 4) reinterpret_cast<int4 *>(slr + (q0 & 1))[tid] = __ldg(reinterpret_cast<const int4 *>(lrp + q0 + 1) + tid);
 	__syncthreads();
 	// FS: pic of the line R1 loads next (q0, then q0 + 1 ...), and of the one after it

@@ -1,8 +1,10 @@
 """The stage after the modulator - IQ swap, the frequency-offset mixer from its start-up, the channel combiner
 (--passthru, htv_render_add) and the store - at every kernel form, against the oracle.
 
-Every emitted sample passes kl_mix + kl_post_store (htv_sound.cuh, htv_line.cuh) in k_line, SECAM's SRC form included, or
-kl_mix<-1, 1> + mod_store (htv_kernels.cu) in k_mod, k_mod_tma, k_mod_mma and k_fmv_mod. Both have width-dependent
+Every emitted sample passes the mixers (htv_sound.cuh: kl_swap and kl_offset, from the line's sound descriptor in kl_mix or
+from the lane state in kl_mix_lane) and a store: kl_post_store (htv_line.cuh) in k_line, SECAM's SRC form included, or
+mod_store (htv_kernels.cu) in k_mod, k_mod_tma, k_mod_mma and k_fmv_mod, both converting other sample types through
+st_put_sum. Both stores have width-dependent
 branches: the partial last tile, the single-warp CTA, mod_store's 128-bit branch (4 | W) and its per-sample one, and
 `acc` stops at acc_rows, which can fall inside a persistent CTA's run of lines. The other device matrices render with the
 stage idle. ROWS: the narrowest row of each (line_kernel, P = 0 or not, complex or real output) of the colour-phase,

@@ -48,6 +48,11 @@ CASES = [
     ("pal-fm_20M_filter_float", "pal-fm", dict(vfilter=True), 20_000_000, 0, {}, "float", 900),
     ("i_16M_filter_split_long", "i", dict(vfilter=True), 16_000_000, 0, SPLIT, "int16", 20_500),
     ("i_16M_filter_default", "i", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
+    # not the compiled-in sound mask: the general k_line form, its mixers from the line's sound descriptor
+    ("i_16M_filter_default_offset_swap", "i", dict(vfilter=True, offset=2_000_000, swap_iq=True), 16_000_000, 0, {},
+     "int16", 1400),
+    # k_line with the generic NICAM sum on every line
+    ("i_10M_default", "i", dict(), 10_000_000, 0, {}, "int16", 1400),
     # the fused line kernel's sound pre-pass and descriptors in the caller's stream order
     ("i_16M_filter_default_no_ahead", "i", dict(vfilter=True), 16_000_000, 0, dict(HTV_AHEAD="0"), "int16", 1400),
     ("l_16M_filter_default", "l", dict(vfilter=True), 16_000_000, 0, {}, "int16", 1400),
